@@ -23,12 +23,21 @@ so the late, badly scaled systems are timed and checked too).
           one full step, timed; no extrapolation.  It runs after the GPU line has been printed
           (and flushed) once, under a wall-clock limit; the completed line is printed last.
 Timing: CUDA events on the library's own stream, max over ranks, W >= 3 warm-up steps.  The
-factor/solve working set (panel storage) is far larger than the 126 MB L2 for every workload
-except C1, so no explicit L2 flush is done ("inputs larger than L2").
+factor/solve working set (panel storage) is larger than the H100's 50 MB L2 for every workload
+except C1 and C4t, so no explicit L2 flush is done ("inputs larger than L2").
+
+--dump-outputs DIR : after the timed steps, the solutions (x, z) of the three solves of the last
+timed device-resident step are written as DIR/x_<k>.npy, DIR/z_<k>.npy (float64).  A vector longer
+than DUMP_MAX entries is replaced by a fixed, seeded sample of them, and the sampled positions are
+written as DIR/<x|z>_index.npy.  The host time of these downloads is taken out of the timed window.
+The replayed systems are recorded from this build's own GPU solve, so the dumps of two builds compare
+output for output only while both take the same IP iterations to the same iterates.  C5 (the default)
+gave bitwise identical dumps in repeated runs of one build; C2 cannot (its root front is assembled with
+FP64 atomics), and builds that differ in rounding may replay slightly different late systems.
 
 --impl reference : the reference's CPU path on the SAME full-size instance (no sampling, no flop
 ratio): the oracle runs the real interior-point iterations and the KKT sections of the first
-iterations are timed.  When a single step costs more than the time budget allows (C5: ~2.5 min
+iterations are timed.  When a single step costs more than the time budget allows (C5: minutes
 per factorisation), the one step that is timed is the solver's own first factorisation
 (solver_default_start!, identity scaling) + 3 solves; `steps` in the line says how many were timed.
 """
@@ -61,6 +70,8 @@ WORKLOADS = {
 ORDERING_NAMES = {0: "amd", 1: "nested-dissection", 2: "natural", 3: "user", 4: "cone-block-dissection"}
 CPU_LEG_LIMIT_S = float(os.environ.get("CB200_CPU_LEG_LIMIT", "330"))      # wall clock, b200 arm
 REF_ARM_BUDGET_S = float(os.environ.get("CB200_REF_BUDGET", "200"))        # timed CPU work, reference arm
+HBM_PEAK_GBS = 3350.0          # NVIDIA H100 SXM data sheet (HBM3, 700 W part); not a measured figure
+DUMP_MAX = 1 << 19             # entries per dumped vector (8 files at most: <= 34 MB in all)
 
 
 def make_problem(name):
@@ -72,9 +83,9 @@ def make_problem(name):
 def workload_config(name, data, N, nnzK):
     """Identical in both arms: what the instance is, nothing about how an arm solves it."""
     gen, kw = WORKLOADS[name]
-    # factor storage per step: C3 0.4 GB, C4 4.2 GB, C5 1.6 GB (>> the 126 MB L2); C1 2 MB, C2 58 MB
-    l2 = ("working set fits in the 126 MB L2 and is NOT flushed between steps (latency-bound parity config)"
-          if name in ("C1", "C2", "C4t") else "inputs larger than L2 (no flush)")
+    # factor storage per step: C3 0.4 GB, C4 4.2 GB, C5 1.6 GB, C2 58 MB (> the 50 MB L2 of an H100); C1 2 MB
+    l2 = ("working set fits in the 50 MB L2 and is NOT flushed between steps (latency-bound parity config)"
+          if name in ("C1", "C4t") else "inputs larger than L2 (no flush)")
     return dict(workload=name, generator=gen, generator_kwargs=kw, n=int(data.n), m=int(data.m),
                 N=int(N), nnzK=int(nnzK), l2=l2)
 
@@ -143,7 +154,7 @@ def pick_replay(steps):
 def sample_clocks(stop, out):
     q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit")
     while not stop.is_set():
         try:
             r = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader,nounits", "-i",
@@ -157,7 +168,7 @@ def sample_clocks(stop, out):
 
 def clocks_summary(samples):
     if not samples:
-        return dict(sm_mhz=None, sm_max_mhz=None, reasons=["unavailable"])
+        return dict(sm_mhz=None, sm_max_mhz=None, power_limit_w=None, reasons=["unavailable"])
     sm = [float(s[1]) for s in samples if len(s) > 2]
     reasons = set()
     names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
@@ -165,9 +176,13 @@ def clocks_summary(samples):
         for k, nm in enumerate(names):
             if len(s) > 5 + k and s[5 + k].lower().startswith("active"):
                 reasons.add(nm)
+    try:
+        power_limit = float(samples[0][9])
+    except (IndexError, ValueError):
+        power_limit = None
     return dict(sm_mhz=float(np.median(sm)) if sm else None,
                 sm_max_mhz=float(samples[0][2]) if len(samples[0]) > 2 else None,
-                reasons=sorted(reasons))
+                power_limit_w=power_limit, reasons=sorted(reasons))
 
 
 def sym_matvec(K):
@@ -297,19 +312,27 @@ def reference_arm(name, steps, warmup):
     return line
 
 
+def _sampled(v, name, out_dir):
+    """v itself, or a fixed seeded sample of DUMP_MAX of its entries (positions saved beside it)"""
+    if len(v) <= DUMP_MAX:
+        return v
+    idx = np.sort(np.random.default_rng(0).choice(len(v), DUMP_MAX, replace=False))
+    np.save(os.path.join(out_dir, f"{name}_index.npy"), idx.astype(np.float64))
+    return v[idx]
+
+
+def dump_outputs(out_dir, sols, n, m):
+    """x_<k>.npy, z_<k>.npy: what kktsolver_solve! hands its caller (lhsx, lhsz) for solve k of the step"""
+    os.makedirs(out_dir, exist_ok=True)
+    for k, xf in enumerate(sols):
+        for name, v in (("x", xf[:n]), ("z", xf[n:n + m])):
+            np.save(os.path.join(out_dir, f"{name}_{k}.npy"), _sampled(np.asarray(v, np.float64), name, out_dir))
+
+
 def _watchdog(seconds):
     """A hung collective must not hang the caller: dump stacks and exit non-zero."""
     import faulthandler
     faulthandler.dump_traceback_later(seconds, exit=True)
-
-
-def load_traffic(name):
-    """ncu dram__bytes of the kernel classes (per call), committed under profiles/ (see
-    profiles/r02_summary.md for the command); None when no capture exists for the workload."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json"))).get(name)
-    except Exception:
-        return None
 
 
 def main():
@@ -321,6 +344,8 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default=os.environ.get("CB200_WORKLOAD", "C5"))
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the solutions of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -385,7 +410,9 @@ def main():
         staged.append((st_t, rhs_t))
     torch.cuda.synchronize()
 
-    def step(i):
+    def step(i, sink=None):
+        """sink: list that receives the host copy of every solution of this step (resident mode); the
+        host seconds the downloads take are added to step.sink_s"""
         k = i % len(replay)
         s_ = replay[k]
         if ks.ldl.resident:
@@ -394,24 +421,31 @@ def main():
             for tx, tz in rhs_t:
                 ks.setrhs_staged(tx.data_ptr() if tx.numel() else 0, tz.data_ptr() if tz.numel() else 0)
                 ok &= ks.solve(None, None)
+                if sink is not None:           # the solve has synchronised: the stream is idle here
+                    t0_ = time.perf_counter()
+                    sink.append(ks.ldl.download(6, N))
+                    step.sink_s += time.perf_counter() - t0_
             return ok
         ok = ks.update(FakeCones(s_["state"]))
         for rx, rz in s_["rhs"]:
             ks.setrhs(rx, rz); ok &= ks.solve(lx, lz)
         return ok
 
-    def timed(nsteps, offset):
+    def timed(nsteps, offset, sink=None):
+        """device ms of `nsteps` steps; with a sink, the last step's solutions are collected into it and
+        the time spent downloading them (the stream is idle meanwhile) is not counted"""
         if world > 1:
             import torch.distributed as dist
             dist.barrier()
         torch.cuda.synchronize()
+        step.sink_s = 0.0
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(stream)
         for i in range(nsteps):
-            step(offset + i)
+            step(offset + i, sink if i == nsteps - 1 else None)
         e1.record(stream)
         torch.cuda.synchronize()
-        ms = e0.elapsed_time(e1)
+        ms = e0.elapsed_time(e1) - 1e3 * step.sink_s
         if world > 1:
             import torch.distributed as dist
             t = torch.tensor([ms], device="cuda", dtype=torch.float64)
@@ -436,7 +470,10 @@ def main():
     for i in range(args.warmup):
         step(i)
     ks.ldl.reset_timers(); ks.ir_rounds = 0; ks.n_solves = 0
-    ms_res = timed(args.steps, args.warmup)
+    last_sols = [] if args.dump_outputs else None
+    ms_res = timed(args.steps, args.warmup, last_sols)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_sols, n, m)
     tm = ks.ldl.timers()
     ir_per_solve = ks.ir_rounds / max(1, ks.n_solves)
     stop.set(); th.join(timeout=2)
@@ -507,16 +544,11 @@ def main():
                   resident_vs_host_rel_diff=res_diff, cpu_rel_diff=None)
     info = ks.ldl.info()
     stats = ks.ldl.stats()
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback (B200_PROFILING.md)"
+    hbm_peak = HBM_PEAK_GBS
+    peak_src = "H100 SXM data sheet, 3.35 TB/s (not measured)"
     nfac, nsol = max(1, tm["nfactor"]), max(1, tm["nsolve"])
     nnzL, nnzK = int(info.nnzL), int(ks.KKT.nnz)
-    # ---- FP64 compute calibration on this box (no FP64 figure in MEASURED_PEAKS.json): cuBLAS DGEMM
+    # ---- FP64 compute calibration on this GPU: a 4096^3 DGEMM through torch
     fp64_peak = None
     try:
         a_ = torch.randn(4096, 4096, dtype=torch.float64, device="cuda")
@@ -541,21 +573,19 @@ def main():
     t_spmv = tm["spmv_ms"] / nsol * 1e-3
     t_schur = td["schur_ms"] / nfd * 1e-3
     rank_flops = stats.get("rank_flops", stats["flops"]) if world > 1 else stats["flops"]
-    traffic = load_traffic(name) or {}
     kernels = dict(
         triangular_solve_sweeps=dict(bound="hbm", ms_per_call=t_solve * 1e3, calls_per_step=nsol / args.steps,
                                      achieved=b_solve / t_solve / 1e9, unit="GB/s", peak=hbm_peak,
-                                     algorithmic_bytes=b_solve, traffic=traffic.get("triangular_solve_sweeps")),
+                                     algorithmic_bytes=b_solve),
         spmv_residual=dict(bound="hbm", ms_per_call=t_spmv * 1e3, calls_per_step=nsol / args.steps,
                            achieved=b_spmv / max(t_spmv, 1e-12) / 1e9, unit="GB/s", peak=hbm_peak,
-                           algorithmic_bytes=b_spmv, traffic=traffic.get("spmv_residual")),
+                           algorithmic_bytes=b_spmv),
         factor_total=dict(bound="fp64", ms_per_call=t_fac * 1e3, calls_per_step=nfac / args.steps,
                           achieved=rank_flops / t_fac / 1e12, unit="TFLOP/s", peak=fp64_peak,
                           algorithmic_flops=rank_flops),
         schur_gemm=dict(bound="fp64", ms_per_call=t_schur * 1e3, calls_per_step=1.0,
                         achieved=(stats["schur_flops"] / t_schur / 1e12) if t_schur > 0 else None,
-                        unit="TFLOP/s", peak=fp64_peak, algorithmic_flops=stats["schur_flops"],
-                        traffic=traffic.get("schur_gemm")),
+                        unit="TFLOP/s", peak=fp64_peak, algorithmic_flops=stats["schur_flops"]),
         factor_pivot_blocks=dict(ms_per_call=td["panel_ms"] / nfd), factor_small_fronts=dict(ms_per_call=td["small_ms"] / nfd),
         factor_assembly=dict(ms_per_call=td["asm_ms"] / nfd))
     for k in kernels.values():
@@ -576,17 +606,17 @@ def main():
     dom = max(cand, key=cand.get)
     kd = kernels[dom]
     roofline = dict(bound=kd["bound"] if kd["bound"] == "hbm" else "tensor", kernel=dom, achieved=kd["achieved"],
-                    peak=kd["peak"], unit=kd["unit"], frac=kd.get("frac"), traffic=kd.get("traffic"),
+                    peak=kd["peak"], unit=kd["unit"], frac=kd.get("frac"),
                     peak_source=(peak_src if kd["bound"] == "hbm" else
-                                 "on-box cuBLAS DGEMM 4096^3 (float64) - MEASURED_PEAKS.json has no FP64 figure"),
-                    note="FP64 throughout: bound 'tensor' means the FP64 tensor-core path (DMMA; tcgen05 has no f64 "
-                         "kind, DESIGN.md section 4) measured against an on-box DGEMM",
+                                 "DGEMM 4096^3 (float64, torch.matmul) timed on the same GPU"),
+                    note="FP64 throughout: bound 'tensor' means the FP64 tensor-core path (DMMA; wgmma has no f64 "
+                         "type, DESIGN.md section 4) measured against a DGEMM on the same GPU",
                     kernels=kernels)
     config = workload_config(name, solver.data, N, nnzK)
     line = dict(metric=METRIC, value=args.steps / (ms_res * 1e-3), unit="it/s", n_gpus=args.gpus,
                 steps=args.steps, warmup=args.warmup, ms_per_step=ms_res / args.steps,
                 higher_is_better=True, scaling="strong", vs_baseline=None, dtype="f64",
-                data="synthetic", impl="b200", config=config,
+                data="synthetic", impl="b200", gpu=torch.cuda.get_device_name(dev), config=config,
                 details=dict(nnzL=nnzL, factor_flops=stats["flops"], nsuper=int(stats["nsuper"]),
                              nlevels=int(stats["nlevels"]),
                              ordering=ORDERING_NAMES.get(int(stats.get("ordering_used", -1)), "?"),

@@ -1,9 +1,9 @@
-"""clarabel.jl_b200 — B200-native KKT linear-system path for Clarabel.jl's interior-point loop.
+"""clarabel.jl_b200 — H100-native KKT linear-system path for Clarabel.jl's interior-point loop.
 
 Scope (SURVEY.md section 8): cone-Hessian -> KKT value update, static regularisation, sparse
 multifrontal LDL' factorisation, triangular solves + iterative refinement, behind the
 reference's AbstractKKTSolver / AbstractDirectLDLSolver plugin interfaces.  The numerics live
-in csrc/ (hand-written sm_100a CUDA + host C++ symbolic analysis) behind the C-ABI declared in
+in csrc/ (hand-written sm_90a CUDA + host C++ symbolic analysis) behind the C-ABI declared in
 include/clarabel_b200.h; the Python modules here are the host-side mirror of the reference's
 interface (the Julia toolchain is absent from this image) and the caller harness.
 """

@@ -227,9 +227,10 @@ struct cb200_handle {
     bool to_large(int nf, int ns) const { return front_is_large(opt, nf, ns); }
     // TMA descriptors of the large-front panels (one CUtensorMap per large front)
     bool use_tma = false; int tma_kmajor = 1;
-    int tma_tile = 64;                // CTA tile of the TMA GEMM: 64 (3 CTAs per SM; measured best on every workload:
-                                      // C5 Schur 5.4 ms against 8.4 with 128 and 7.5 with the LDG kernel, C4 32 / 42.5 / 42.9),
-                                      // 128, or 0 = by front size (CB200_TMA_TILE)
+    int reduce_blocks = 1;            // grid cap of the grid-stride max-reductions: 8 CTAs per SM of the device
+    int tma_tile = 64;                // CTA tile of the TMA GEMM: 64 (3 CTAs per SM, 64 KB of shared memory each; the
+                                      // fastest on the H100, DESIGN.md section 4), 128 (1 CTA per SM, spills on sm_90a),
+                                      // or 0 = by front size (CB200_TMA_TILE)
     DevBuf<CUtensorMap> d_tmaps, d_tmaps64; DevBuf<int32_t> d_tmap_of;
     // multi-GPU state
     bool dist = false; int rank = 0, nranks = 1;
@@ -249,11 +250,11 @@ struct cb200_handle {
     bool multi_stream = true;
     bool sort_batches = true;          // CB200_SORT_BATCHES=0: keep the size order of the level lists
     bool merged_rows = true;           // 16-column warp solve kernels fetch the triangle and the first L21 chunk in ONE batch
-                                       // of loads (one dependent round trip less; 80 registers, 3 CTAs/SM).  Measured on
-                                       // C5 / C3: fwd -8 % / -5 %, bwd -10 % / -7 %.  CB200_MERGED_ROWS=0: two-phase loads.
+                                       // of loads (one dependent round trip less; 80 registers, 3 CTAs/SM).
+                                       // CB200_MERGED_ROWS=0: two-phase loads.
     // bottom subtrees of narrow supernodes solved by one CTA each (k_fwd_subtree / k_bwd_subtree)
-    bool use_subtree = false;          // CB200_SUBTREE=1 turns them on.  Measured (C5): 5.58 ms per solve against 3.19 ms
-                                       // level-scheduled - with only L streamed from HBM but metadata still fetched per
+    bool use_subtree = false;          // CB200_SUBTREE=1 turns them on.  Slower than the level-scheduled kernels
+                                       // - with only L streamed from HBM but metadata still fetched per
                                        // supernode, 16 warps per SM are too few to hide the dependent round trips.  Kept as
                                        // the base of a version that bulk-prefetches the (contiguous) subtree panels.
     int32_t nsub = 0, sub_nlev = 0, sub_maxcols = 0, sub_maxrows = 0;
@@ -731,7 +732,7 @@ int factor_body(cb200_handle* h, bool static_reg) {
     if (h->nnzK) { k_scatter<<<nblk(h->nnzK, 256), 256, 0, st>>>(h->d_nz.p, h->d_amap.p, h->nnzK, h->d_L.p); LAUNCH(h); }
     if (static_reg && h->st.static_regularization_enable && h->N) {
         CUDA_OK(cudaMemsetAsync(h->d_scal.p, 0, sizeof(unsigned long long), st));
-        k_diag_absmax<<<std::min(nblk(h->N, 256), 1184), 256, 0, st>>>(h->d_nz.p, h->d_diagidx.p, h->N, h->d_scal.p);
+        k_diag_absmax<<<std::min(nblk(h->N, 256), h->reduce_blocks), 256, 0, st>>>(h->d_nz.p, h->d_diagidx.p, h->N, h->d_scal.p);
         k_compute_eps<<<1, 1, 0, st>>>(h->d_scal.p, h->st.static_regularization_constant,
                                        h->st.static_regularization_proportional, h->d_eps.p);
         k_shift_diag<<<nblk(h->N, 256), 256, 0, st>>>(h->d_nz.p, h->d_diagidx.p, h->d_amap.p,
@@ -1026,6 +1027,7 @@ int32_t cb200_create(int64_t N, const int64_t* colptr, const int64_t* rowval, co
         g_block_hint.clear();
         const Symbolic& S = h->S;
         CUDA_OK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+        { int nsm = 0; CUDA_OK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, h->st.device)); h->reduce_blocks = 8 * nsm; }
         for (int i = 0; i < 3; ++i) {
             CUDA_OK(cudaStreamCreateWithFlags(&h->side[i], cudaStreamNonBlocking));
             CUDA_OK(cudaEventCreateWithFlags(&h->ev_join[i], cudaEventDisableTiming));
@@ -1205,7 +1207,7 @@ int32_t cb200_scale_values(cb200_handle* h, const int64_t* index, int64_t len, d
 static int finish_factor(cb200_handle* h) {
     // success = all(isfinite, Dinv)   (directldl_qdldl.jl:79)
     CUDA_OK(cudaMemsetAsync(h->d_scal.p + 3, 0, sizeof(unsigned long long), h->stream));
-    if (h->N) { k_absmax<<<std::min(nblk(h->N, 256), 1184), 256, 0, h->stream>>>(h->d_Dinv.p, h->N, h->d_scal.p + 3); LAUNCH(h); }
+    if (h->N) { k_absmax<<<std::min(nblk(h->N, 256), h->reduce_blocks), 256, 0, h->stream>>>(h->d_Dinv.p, h->N, h->d_scal.p + 3); LAUNCH(h); }
     if (h->dist) {
         // every rank must take the same success / failure branch: reduce the status over the ranks
         // (the value is the bit pattern of a non-negative double, so unsigned max == double max)
@@ -1422,7 +1424,7 @@ int32_t cb200_solve_ir(cb200_handle* h, const double* rhsx, const double* rhsz,
     }
     k_build_rhs<<<nblk(N, 256), 256, 0, st>>>(h->d_rx.p, h->d_rz.p, n, m, N, h->d_b.p);
     CUDA_OK(cudaMemsetAsync(h->d_scal.p + 1, 0, sizeof(unsigned long long), st));
-    k_absmax<<<std::min(nblk(N, 256), 1184), 256, 0, st>>>(h->d_b.p, N, h->d_scal.p + 1);
+    k_absmax<<<std::min(nblk(N, 256), h->reduce_blocks), 256, 0, st>>>(h->d_b.p, N, h->d_scal.p + 1);
     h->tm.nlaunch += 2;
     double* x = h->d_x.p; double* dx = h->d_dx.p; double* e = h->d_e.p;
     int rc = tri_solve(h, h->d_b.p, x);
@@ -1455,7 +1457,7 @@ int32_t cb200_solve_ir(cb200_handle* h, const double* rhsx, const double* rhsz,
         }
     } else {
         CUDA_OK(cudaMemsetAsync(h->d_scal.p + 2, 0, sizeof(unsigned long long), st));
-        k_absmax<<<std::min(nblk(N, 256), 1184), 256, 0, st>>>(x, N, h->d_scal.p + 2); LAUNCH(h);
+        k_absmax<<<std::min(nblk(N, 256), h->reduce_blocks), 256, 0, st>>>(x, N, h->d_scal.p + 2); LAUNCH(h);
         double sc[1];
         rc = read_scalars(h, sc, 2, 1); if (rc) return rc;
         ok = std::isfinite(sc[0]);

@@ -1,4 +1,4 @@
-// Device kernels for the B200 KKT path (sm_100a).  FP64 throughout (the reference is Float64
+// Device kernels for the H100 KKT path (sm_90a).  FP64 throughout (the reference is Float64
 // end-to-end and its IR tolerance is 1e-13 - src/settings.jl:127-132).
 //
 //   G1  cone -> K value update            k_hs_diag, k_hs_soc_dense, k_soc_expansion, k_soc_D
@@ -227,7 +227,7 @@ k_factor_panel(DevSym S, const int32_t* __restrict__ batch, int maxpanel, int ma
         if (wid == 0) {
             // right-looking LDL' of the cbk x cbk diagonal sub-block in shared memory, lane j owns column
             // kb + j.  (The former register/shuffle version sat inside a loop whose bounds the compiler cannot
-            // prove warp-uniform: every shuffle became a WARPSYNC.COLLECTIVE, ~50 cycles each.)
+            // prove warp-uniform: every shuffle became a WARPSYNC.COLLECTIVE, tens of cycles each.)
             for (int k = 0; k < cbk; ++k) {
                 double d = P[(kb + k) + (kb + k) * nf];
                 const double sg = (double)S.dsign[f + kb + k];
@@ -431,7 +431,7 @@ k_assemble_atomic(DevSym S, int s, double* __restrict__ Lst, double* __restrict_
 // k_ldl_update exists in two versions:
 //   k_ldl_update_tma   128 x 128 CTA tile, operands brought in by TMA (cp.async.bulk.tensor.3d) through a
 //                      4-stage mbarrier ring by one producer warp, 8 consumer warps on the FP64
-//                      tensor-core path (DMMA m8n8k4; tcgen05 has no f64 kind)
+//                      tensor-core path (DMMA; wgmma has no f64 type)
 //   k_ldl_update_ldg   64 x 64 tile, LDG -> registers -> STS double buffering (fallback when the
 //                      driver cannot encode tensor maps, and the reference for A/B comparisons)
 constexpr int GBM = 64, GBK = 16;
@@ -720,9 +720,9 @@ k_ldl_update_tma(DevSym S, const int32_t* __restrict__ batch, const CUtensorMap*
         mbar_wait(full + st, ph);
         // Release of the PREVIOUS stage, one iteration late and after the wait above.  Releasing a stage at
         // the end of its own iteration is not safe: ptxas schedules the SYNCS.ARRIVE right behind the last
-        // LDS *issue* (before the DMMAs that consume them - it did, see profiles/r02_tma_release_race.md),
+        // LDS *issue* (before the DMMAs that consume them - it did, DESIGN.md section 4),
         // the arrive does not wait for loads in flight, and with 3 CTAs per SM an LDS can be overtaken by
-        // the TMA refill of its stage: ~1 corrupted tile per 1e6, 3-5 % of the C4r factorisations.  Here
+        // the TMA refill of its stage: rare corrupted tiles, seen on sm_100a.  Here
         // every DMMA of stage it-1 was issued before the spin-wait (they cannot sink below its loop), a DMMA
         // issues only when its LDS operands have arrived, and the arrive cannot rise above the acquire.
         if (it > 0) {
@@ -731,20 +731,23 @@ k_ldl_update_tma(DevSym S, const int32_t* __restrict__ batch, const CUtensorMap*
         }
         const double* A = sA + st * TTILE + (wm / 8) * srg + g;
         const double* B = sB + st * TTILE + (wn / 8) * srg + g;
-        double bf[NJ][4];
+        // All A fragments stay live while the B fragments stream past them one n8 tile at a time
+        // (MI x 8 + 4 doubles).  Holding all NJ B fragments instead made sm_90a spill the T = 64 loop
+        // under its 3-CTA/SM budget of 128 registers.
+        double af[MI][8];
 #pragma unroll
-        for (int j = 0; j < NJ; ++j)
-#pragma unroll
-            for (int v = 0; v < 4; ++v) bf[j][v] = B[j * srg + (4 * v + t) * sk] * dv[v];
-#pragma unroll
-        for (int i = 0; i < MI; ++i) {
-            double af[8];
+        for (int i = 0; i < MI; ++i)
 #pragma unroll
             for (int v = 0; v < 4; ++v)
 #pragma unroll
-                for (int h = 0; h < 2; ++h) af[2 * v + h] = A[(2 * i + h) * srg + (4 * v + t) * sk];
+                for (int h = 0; h < 2; ++h) af[i][2 * v + h] = A[(2 * i + h) * srg + (4 * v + t) * sk];
 #pragma unroll
-            for (int j = 0; j < NJ; ++j) dmma16816(acc[i][j], af, bf[j]);
+        for (int j = 0; j < NJ; ++j) {
+            double bf[4];
+#pragma unroll
+            for (int v = 0; v < 4; ++v) bf[v] = B[j * srg + (4 * v + t) * sk] * dv[v];
+#pragma unroll
+            for (int i = 0; i < MI; ++i) dmma16816(acc[i][j], af[i], bf);
         }
     }
     // ===== epilogue: subtract into the panel (col < ns) or the update block.  All loads of a column
@@ -1055,7 +1058,7 @@ __device__ __forceinline__ double row_dot64(const double* __restrict__ rowp, int
 // (warp-level; result valid on all lanes after the shuffles)
 // Sum 8 per-lane partial sums over the warp through shared memory: lane u (< 8) returns sum_u.
 // (Shuffle trees inside loops whose trip count comes from memory are wrapped in WARPSYNC.COLLECTIVE
-// on sm_100a; `red` is 8 x 33 doubles owned by the warp.)
+// by the compiler; `red` is 8 x 33 doubles owned by the warp.)
 __device__ __forceinline__ double warp_sum8_smem(const double (&a)[8], double* red, int lane) {
 #pragma unroll
     for (int u = 0; u < 8; ++u) red[u * 33 + lane] = a[u];
@@ -1238,7 +1241,7 @@ __device__ __forceinline__ void fwd_warp_body(const SnView& V, double* Y, double
 // window Y, all others (ancestors outside a subtree) from the global solution vector yg.
 // The transposed products go through a 32 x (NW+1) shared tile (coalesced loads by rows, conflict-free
 // reads by columns) instead of shuffle reductions: inside the loops of the subtree kernel the compiler
-// cannot prove warp convergence and wraps every shuffle in WARPSYNC.COLLECTIVE (~50 cycles each).
+// cannot prove warp convergence and wraps every shuffle in WARPSYNC.COLLECTIVE (tens of cycles each).
 constexpr int BT_LD = 33;
 template <int NW>
 __device__ __forceinline__ void bwd_warp_body(const SnView& V, const double* __restrict__ Dinv, double* Y,
@@ -1556,8 +1559,8 @@ k_bwd_cta(DevSym S, const int32_t* __restrict__ batch, const double* __restrict_
     extern __shared__ double w[];
     __shared__ double ts[SB];
     __shared__ double red8[8][8 * 33];
-    // (the packed descriptors of the warp kernels were measured here too: 13 % slower on C5 - the per-supernode
-    // index arrays are L2-resident, the 64-byte descriptors are not)
+    // (the packed descriptors of the warp kernels were measured slower here: the per-supernode index arrays
+    // are L2-resident, the 64-byte descriptors are not)
     const int s = batch[blockIdx.x];
     const int f = S.sn_first[s];
     const int ns = S.sn_first[s + 1] - f;

@@ -2,7 +2,7 @@
 //
 // The reference obtains its ordering from AMD.jl -> SuiteSparse AMD inside QDLDL.jl
 // (reference call site: src/kktsolvers/direct-ldl/directldl_qdldl.jl:18-25, with
-// amd_dense_scale = 1.5).  Neither library is in /root/reference or in this image, so this
+// amd_dense_scale = 1.5).  Neither library is part of the Clarabel.jl repository, so this
 // file restates the published algorithm (Amestoy, Davis, Duff, "An approximate minimum degree
 // ordering algorithm", SIMAX 1996): quotient graph, element absorption, approximate external
 // degree, mass elimination, supervariable detection by hashing, aggressive absorption and

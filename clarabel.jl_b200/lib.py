@@ -50,7 +50,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"{LIB_PATH} is missing: build it with __graft_entry__.build() "
-                "(nvcc, sm_100a).  The B200 backend has no CPU fallback.")
+                "(nvcc, sm_90a).  The CUDA backend has no CPU fallback.")
         L = C.CDLL(LIB_PATH)
         I64, I32, D, P = C.c_int64, C.c_int32, C.c_double, C.c_void_p
         L.cb200_default_settings.argtypes = [P]

@@ -1,11 +1,11 @@
-/* clarabel_b200.h — C-ABI of the B200-native KKT linear-system backend for Clarabel.jl.
+/* clarabel_b200.h — C-ABI of the CUDA (H100, sm_90a) KKT linear-system backend for Clarabel.jl.
  *
  * Drop-in boundary (SURVEY.md section 8b).  Two reference interfaces are covered:
  *
  *  (1) INNER = the reference's LDL plugin API `AbstractDirectLDLSolver`
- *      (/root/reference/src/kktsolvers/direct-ldl/directldl_defaults.jl:1-72; the QDLDL
+ *      (Clarabel.jl/src/kktsolvers/direct-ldl/directldl_defaults.jl:1-72; the QDLDL
  *      implementation it replaces is directldl_qdldl.jl:1-96).  One C function per method.
- *  (2) OUTER = `AbstractKKTSolver` (/root/reference/src/kktsolvers/kktsolver_defaults.jl:1-47,
+ *  (2) OUTER = `AbstractKKTSolver` (Clarabel.jl/src/kktsolvers/kktsolver_defaults.jl:1-47,
  *      concrete reference implementation kktsolver_directldl.jl), fused so that cone state is
  *      uploaded once per iteration and the cone->K update, static regularisation,
  *      factorisation, solves and iterative refinement all run on the device.

@@ -22,7 +22,10 @@ def build(force=False):
 def lib():
     global _LIB
     if _LIB is None:
-        L = C.CDLL(build())
+        so = os.path.join(_HERE, "liboracle.so")
+        # rebuilt when stale; a tree that cannot be written to (a read-only checkout the benchmark runs
+        # from) uses the library build() left there
+        L = C.CDLL(build() if os.access(_HERE, os.W_OK) or not os.path.exists(so) else so)
         I, D, P = C.c_int64, C.c_double, C.c_void_p
         L.qdldl_oracle_new.restype = P
         L.qdldl_oracle_new.argtypes = [I, P, P, P, P, P, D, D, C.c_int]

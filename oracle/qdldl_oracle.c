@@ -1,7 +1,7 @@
 /* TEST INFRASTRUCTURE ONLY — CPU oracle, never imported by the product path.
  *
  * Restatement of the LDL' engine the reference calls for its KKT path: QDLDL.jl (pure Julia,
- * compat "0.4.1" at /root/reference/Project.toml:38 — NOT vendored under /root/reference, so
+ * compat "0.4.1" at Clarabel.jl/Project.toml:38 — NOT vendored under the Clarabel.jl repository, so
  * "parity unpinned" at this boundary; see DESIGN.md).  The algorithm restated is the published
  * QDLDL one (Stellato et al., OSQP / QDLDL: elimination tree + up-looking sparse LDL' for
  * quasidefinite matrices, after Davis' LDL) with the additions QDLDL.jl makes and the reference

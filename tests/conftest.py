@@ -9,7 +9,7 @@ for p in (ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tests", "golden
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 @pytest.fixture(scope="session")

@@ -1,5 +1,5 @@
 """Golden known-answer cases transcribed from the reference's own end-to-end tests
-(/root/reference/test/OptTests/*.jl).  Problem data and expected answers are the literals in
+(Clarabel.jl/test/OptTests/*.jl).  Problem data and expected answers are the literals in
 those files (file:line cited per case); the reference asserts them at atol = 1e-3.
 
 Each case: dict(name, P, q, A, b, cones, status, x=None, obj=None, obj_dual=None).

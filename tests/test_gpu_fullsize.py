@@ -1,4 +1,4 @@
-"""GPU parity at the BASELINE.json sizes (run with -m gpu on the B200 box).
+"""GPU parity at the BASELINE.json sizes (run with -m gpu on an H100).
 
 north_star: "results must match the reference QDLDL path on the same problems (primal/dual
 objective and residuals within 1e-6 relative; identical status codes)".  The template is the

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): the CUDA path through the C-ABI against
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path through the C-ABI against
 the CPU oracle on the same seeded inputs.
 
 Tolerances: cone->K value update is pure elementwise FP64 => bit-exact for Zero/NN/SOC blocks

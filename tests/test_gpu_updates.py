@@ -9,6 +9,5 @@ pytestmark = pytest.mark.gpu
 
 @pytest.mark.parametrize("scenario", SCENARIOS)
 def test_data_updating_b200_backend(cb, scenario):
-    # verified on the B200 at 1e-6 (profiles/r01_pytest_gpu_nonsym_updates.log); the reference's
-    # 1e-7 is what the CPU variant in test_caller_paths.py asserts
+    # 1e-6 on the GPU; the reference's 1e-7 is what the CPU variant in test_caller_paths.py asserts
     run_scenario(cb, "b200", scenario, tol=1e-6)

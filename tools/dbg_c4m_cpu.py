@@ -1,6 +1,7 @@
 """CPU check of orderings on a late-iteration SDP KKT matrix: AMD vs ND vs ND with cone blocks kept
 whole, through the numpy multifrontal emulation and the QDLDL oracle (same permutation)."""
-import sys; sys.path.insert(0,'/root/repo'); sys.path.insert(0,'/root/repo/tests')
+import os; ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import sys; sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
 import numpy as np
 import clarabel_jl_b200 as cb
 from clarabel_jl_b200 import lib

@@ -1,4 +1,5 @@
-import sys; sys.path.insert(0,'/root/repo'); sys.path.insert(0,'/root/repo/tests')
+import os; ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import sys; sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
 import numpy as np
 import clarabel_jl_b200 as cb
 from oracle.kktsolver_oracle import OracleDirectLDLKKTSolver

@@ -4,7 +4,7 @@
 
 Uses cb200_set_detail(h, 2): CUDA events around every launch group, graph replay off, so the sum is
 a little above the bench's ms_per_step; the SHARES are what to read.  One table per workload, also
-written as JSON to gpurun_out/fine_<workload>.json when that directory exists."""
+written as JSON to $FINE_OUT/fine_<workload>.json when FINE_OUT names a directory."""
 import json
 import os
 import sys
@@ -50,8 +50,8 @@ def run(name, nsteps=3):
           f"({tm['nsolve'] / nsteps:.1f} sweeps), spmv {tm['spmv_ms'] / nsteps:.2f} ms, launches {tm['nlaunch'] / nsteps:.0f}")
     for k, v in sorted(per.items(), key=lambda kv: -kv[1]):
         print(f"   {k:24s} {v:9.3f} ms  {100 * v / tot:5.1f} %")
-    out = os.path.join(ROOT, "gpurun_out")
-    if os.path.isdir(out):
+    out = os.environ.get("FINE_OUT")
+    if out and os.path.isdir(out):
         json.dump({"workload": name, "ms_per_step": per, "coarse": {k: float(v) / nsteps for k, v in tm.items()},
                    "stats": st}, open(os.path.join(out, f"fine_{name}.json"), "w"), indent=1)
 

@@ -1,5 +1,6 @@
 """Dev tool: run whole IP solves through the b200 backend and print per-phase device times."""
-import sys, time; sys.path.insert(0,'/root/repo')
+import os; ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import sys, time; sys.path.insert(0, ROOT)
 import numpy as np
 import clarabel_jl_b200 as cb
 from clarabel_jl_b200 import problems as pr

@@ -1,4 +1,5 @@
-import sys, time; sys.path.insert(0,'/root/repo')
+import os; ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import sys, time; sys.path.insert(0, ROOT)
 import numpy as np
 import clarabel_jl_b200 as cb
 from clarabel_jl_b200 import lib, problems as pr, kkt_assembly as ka
