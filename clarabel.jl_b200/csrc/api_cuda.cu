@@ -1619,10 +1619,12 @@ int32_t cb200_get_stats(const cb200_handle* h, double* out, int32_t len) {
         }
         if (nf * ns >= 65536 && ns > 32) big_bytes += 8.0 * nf * ns;
     }
-    double v[14] = {S.flops, schur, panel_large - schur, (double)S.nnzL, (double)S.nlevels, (double)S.nsuper,
+    double v[17] = {S.flops, schur, panel_large - schur, (double)S.nnzL, (double)S.nlevels, (double)S.nsuper,
                     nlarge, big_bytes, (double)S.upd_total * 8.0, (double)S.panel_off.back() * 8.0,
-                    (double)S.ordering_used, my_flops, h->use_tma ? 1.0 : 0.0, (double)h->tma_kmajor};
-    for (int i = 0; i < len && i < 14; ++i) out[i] = v[i];
+                    (double)S.ordering_used, my_flops, h->use_tma ? 1.0 : 0.0, (double)h->tma_kmajor,
+                    (double)((h->g_factor[0].exec != nullptr) + (h->g_factor[1].exec != nullptr)),
+                    h->g_solve.exec ? 1.0 : 0.0, (double)h->nsub};
+    for (int i = 0; i < len && i < 17; ++i) out[i] = v[i];
     return 0;
 }
 

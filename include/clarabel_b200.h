@@ -163,7 +163,10 @@ int32_t cb200_get_fine_timers(cb200_handle* h, double* out_ms, int32_t len);
 const char* cb200_fine_timer_name(int32_t i);
 /* symbolic statistics: 0 factor flops (sum of squared column lengths), 1 flops of the large-front
  * Schur GEMMs, 2 flops of the large-front panel phase, 3 nnzL, 4 levels, 5 supernodes, 6 large
- * fronts, 7 panel bytes of the multi-CTA solve class, 8 update-storage bytes, 9 panel-storage bytes */
+ * fronts, 7 panel bytes of the multi-CTA solve class, 8 update-storage bytes, 9 panel-storage bytes,
+ * 10 ordering used, 11 flops of this rank's fronts, 12 TMA tensor maps in use, 13 their k-major order,
+ * 14 factorisation graphs instantiated (0-2), 15 solve-sweep graph instantiated, 16 bottom subtrees
+ * solved by k_fwd_subtree / k_bwd_subtree */
 int32_t cb200_get_stats(const cb200_handle* h, double* out, int32_t len);
 /* ---------------------------------------------------------------- multi-GPU (one process per GPU)
  * Every rank creates the same handle on its own device (replicated symbolic analysis), then

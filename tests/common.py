@@ -40,3 +40,25 @@ def kkt_fixture(cb, gen, seed=0):
 
 def sym_full(K):
     return (K + sp.triu(K, 1).T).tocsc()
+
+
+def random_quasidefinite(seed):
+    """Randomised KKT structures the instance generators do not produce: empty P, empty rows/columns
+    of A, disconnected blocks, dense rows/columns, tiny and degenerate sizes.  -> (K triu CSC, Dsigns)"""
+    rng = np.random.default_rng(1000 + seed)
+    n = int(rng.integers(1, 60)); m = int(rng.integers(0, 80))
+    dens = float(rng.choice([0.02, 0.1, 0.4]))
+    rs = np.random.RandomState(seed)
+    Ph = sp.random(n, n, dens, random_state=rs)
+    P = (Ph @ Ph.T + sp.identity(n) * (0.5 if seed % 3 else 1.0)).tocsc() if seed % 5 else sp.identity(n, format="csc")
+    A = sp.random(m, n, dens, random_state=rs).tolil()
+    if m > 3 and n > 3:
+        A[0, :] = 1.0 if seed % 2 else 0.0                      # dense or empty row
+        A[:, 0] = 0.0                                           # empty column
+        if seed % 4 == 0:
+            A[m // 2:, : n // 2] = 0.0; A[: m // 2, n // 2:] = 0.0      # two disconnected blocks
+    A = A.tocsc()
+    K = sp.bmat([[P, A.T], [A, -sp.identity(m) * 0.7]]).tocsc() if m else P
+    K = sp.triu(K).tocsc(); K.sort_indices()
+    Ds = np.r_[np.ones(n, dtype=np.int64), -np.ones(m, dtype=np.int64)]
+    return K, Ds, rng

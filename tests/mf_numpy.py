@@ -1,7 +1,13 @@
 """Test helper: numpy emulation of the multifrontal numeric phase on the product's symbolic
 structures (panels, update blocks, a_map, rel).  It exercises exactly the index maps the CUDA
-kernels use, so symbolic-analysis bugs are caught on the CPU.  Not part of the product."""
+kernels use, so symbolic-analysis bugs are caught on the CPU.  Not part of the product.
+
+With dtype=np.longdouble (x87 extended precision, 64-bit mantissa) it is the high-precision
+reference the GPU kernel tests compare with: `gpu_storage` converts its factor into the exact
+layout the kernels leave in device memory."""
 import numpy as np
+
+SB = 64          # width of the inverted diagonal blocks of L11 (kernels.cuh: SB == PB)
 
 
 def panel_view(L, s, sn, nf, ns):
@@ -13,26 +19,30 @@ def panel_view(L, s, sn, nf, ns):
 
 
 class MFNumpy:
-    def __init__(self, sym):
+    def __init__(self, sym, dtype=np.float64):
         """sym: dict of arrays from cb200_symbolic_get (see lib.Symbolic.arrays())."""
         self.s = sym
         self.N = len(sym["perm"])
         self.nsuper = len(sym["sn_first"]) - 1
+        self.dtype = dtype
 
-    def factor(self, nzval, dsigns_orig, eps=1e-13, delta=2e-7):
-        s = self.s
-        L = np.zeros(int(s["panel_off"][-1]))
-        U = np.zeros(int(s["upd_off"][-1]))
-        np.add.at(L, s["a_map"], nzval)
-        D = np.zeros(self.N)
+    def factor(self, nzval, dsigns_orig, eps=1e-13, delta=2e-7, enable=True):
+        """LDL' with QDLDL's sign rule: if D[k]*sign < eps then D[k] = delta*sign (when enabled).
+        Counts the replaced pivots (nreg) and records their ORIGINAL indices (reglog, in order)."""
+        s, T = self.s, self.dtype
+        L = np.zeros(int(s["panel_off"][-1]), dtype=T)
+        U = np.zeros(int(s["upd_off"][-1]), dtype=T)
+        np.add.at(L, s["a_map"], np.asarray(nzval, dtype=np.float64).astype(T))
+        D = np.zeros(self.N, dtype=T)
         dsp = np.asarray(dsigns_orig)[s["perm"]]
-        self.nreg = 0
+        eps, delta = T(eps), T(delta)
+        self.nreg, self.reglog = 0, []
         for sn in range(self.nsuper):
             f, l = int(s["sn_first"][sn]), int(s["sn_first"][sn + 1])
             ns = l - f
             nr = int(s["rows_ptr"][sn + 1] - s["rows_ptr"][sn])
             nf = ns + nr
-            F = np.zeros((nf, nf))
+            F = np.zeros((nf, nf), dtype=T)
             F[:, :ns] = panel_view(L, s, sn, nf, ns).T
             for c in s["children"][sn]:
                 nrc = int(s["rows_ptr"][c + 1] - s["rows_ptr"][c])
@@ -41,8 +51,9 @@ class MFNumpy:
                 F[np.ix_(rel, rel)] += np.tril(Uc)
             for k in range(ns):
                 d = F[k, k]
-                if d * dsp[f + k] < eps:
+                if enable and d * dsp[f + k] < eps:
                     d = delta * dsp[f + k]; self.nreg += 1
+                    self.reglog.append(int(s["perm"][f + k]))
                 D[f + k] = d
                 col = F[k + 1:, k].copy()
                 F[k + 1:, k] = col / d
@@ -56,7 +67,7 @@ class MFNumpy:
 
     def solve(self, b):
         s = self.s
-        y = np.asarray(b, dtype=float)[s["perm"]].copy()
+        y = np.asarray(b, dtype=np.float64).astype(self.dtype)[s["perm"]].copy()
         # forward (right-looking form; equivalent to the multifrontal form the kernels use)
         for sn in range(self.nsuper):
             f, l = int(s["sn_first"][sn]), int(s["sn_first"][sn + 1])
@@ -77,6 +88,40 @@ class MFNumpy:
             y[f:l] -= P[ns:, :].T @ y[rows]
             for k in range(ns - 1, -1, -1):
                 y[f + k] -= P[k + 1:ns, k] @ y[f + k + 1:l]
-        x = np.empty(self.N)
+        x = np.empty(self.N, dtype=self.dtype)
         x[s["perm"]] = y
         return x
+
+
+def invert_unit_lower(T):
+    """Inverse of a unit-lower-triangular block by row-wise forward substitution, in T's dtype
+    (numpy's LAPACK path would round a longdouble block to double)."""
+    n = T.shape[0]
+    X = np.zeros_like(T)
+    for i in range(n):
+        X[i, i] = 1
+        if i:
+            X[i, :i] = -(T[i, :i] @ X[:i, :i])
+    return X
+
+
+def gpu_storage(mf):
+    """The factor of `mf` in the device storage format of the panels (DESIGN.md section 3): every
+    supernode's nf x ns panel column-major at panel_off with leading dimension panel_ld, D on the
+    diagonal, and each diagonal block of L11 of up to SB columns (blocks start at column 0 of the
+    supernode) replaced by the inverse of its unit-lower factor, computed in mf's dtype.  Entries
+    above the diagonal of L11 and rows nf..ld-1 are set to 0; the kernels make no promise about
+    the former (see the GPU tests) and leave the padding rows zero."""
+    s = mf.s
+    out = np.zeros_like(mf.L)
+    for sn in range(mf.nsuper):
+        f, l = int(s["sn_first"][sn]), int(s["sn_first"][sn + 1])
+        ns = l - f
+        nf = ns + int(s["rows_ptr"][sn + 1] - s["rows_ptr"][sn])
+        P = np.tril(panel_view(mf.L, s, sn, nf, ns).T)          # nf x ns, unit diagonal
+        for b0 in range(0, ns, SB):
+            b1 = min(ns, b0 + SB)
+            P[b0:b1, b0:b1] = invert_unit_lower(P[b0:b1, b0:b1])
+        P[np.arange(ns), np.arange(ns)] = mf.D[f:l]
+        panel_view(out, s, sn, nf, ns)[:, :] = P.T
+    return out

@@ -6,7 +6,7 @@ import numpy as np
 import scipy.sparse as sp
 import scipy.sparse.linalg as spl
 import pytest
-from common import small_instances, kkt_fixture, sym_full
+from common import small_instances, kkt_fixture, sym_full, random_quasidefinite
 from mf_numpy import MFNumpy
 
 
@@ -144,23 +144,8 @@ def test_symbolic_maps_on_random_quasidefinite_patterns(seed):
     A, disconnected blocks, dense rows/columns, tiny and degenerate sizes; both orderings.  The
     numpy multifrontal runs on exactly the maps the CUDA kernels consume."""
     from clarabel_jl_b200 import lib
-    rng = np.random.default_rng(1000 + seed)
-    n = int(rng.integers(1, 60)); m = int(rng.integers(0, 80))
-    dens = float(rng.choice([0.02, 0.1, 0.4]))
-    rs = np.random.RandomState(seed)
-    Ph = sp.random(n, n, dens, random_state=rs)
-    P = (Ph @ Ph.T + sp.identity(n) * (0.5 if seed % 3 else 1.0)).tocsc() if seed % 5 else sp.identity(n, format="csc")
-    A = sp.random(m, n, dens, random_state=rs).tolil()
-    if m > 3 and n > 3:
-        A[0, :] = 1.0 if seed % 2 else 0.0                      # dense or empty row
-        A[:, 0] = 0.0                                           # empty column
-        if seed % 4 == 0:
-            A[m // 2:, : n // 2] = 0.0; A[: m // 2, n // 2:] = 0.0      # two disconnected blocks
-    A = A.tocsc()
-    K = sp.bmat([[P, A.T], [A, -sp.identity(m) * 0.7]]).tocsc() if m else P
-    K = sp.triu(K).tocsc(); K.sort_indices()
-    N = n + m
-    Ds = np.r_[np.ones(n, dtype=np.int64), -np.ones(m, dtype=np.int64)]
+    K, Ds, rng = random_quasidefinite(seed)
+    N = K.shape[0]
     Kf = sym_full(K)
     b = rng.standard_normal(N)
     xs = np.linalg.solve(Kf.toarray(), b)
