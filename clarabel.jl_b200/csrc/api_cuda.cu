@@ -62,6 +62,9 @@ template <class T> struct DevBuf {
 struct Batch { int32_t off = 0, cnt = 0, maxnf = 0, maxns = 0, maxnr = 0, maxpanel = 0; bool many_children = false;
                int32_t schur_t128 = 0, schur_t64 = 0;
                int32_t src_per_row = 0;
+               // big solve class: the 64-blocks of L11 (forward ticket order, then backward) and the 64-row
+               // tiles of L21 in d_bigwork, and the tickets + ready flags in d_bigsync (build_plans)
+               int32_t work_off = 0, nwork = 0, tile_off = 0, ntile = 0; int64_t sync_off = 0;
                bool all_padded = true;
                std::vector<int32_t> ns_desc;  // large batches are sorted by pivot width (descending): the fronts still
                                               // active at pivot column kb are the first active(kb) of the batch
@@ -186,6 +189,8 @@ struct cb200_handle {
     DevBuf<int32_t> d_asm_colptr, d_asm_src, d_asm_child;
     // numeric
     DevBuf<double> d_L, d_U, d_W, d_D, d_Dinv, d_uvec, d_partial;
+    DevBuf<BigItem> d_bigwork;
+    DevBuf<unsigned> d_bigsync;         // [0]: error word of the current solve call, then per big batch: tickets, flags
     DevBuf<double> d_b, d_x, d_e, d_dx, d_y, d_rx, d_rz;
     DevBuf<double> d_eps; DevBuf<unsigned long long> d_scal;   // [0] max|diag|, [1] normb, [2] norme
     DevBuf<unsigned int> d_nreg; DevBuf<int32_t> d_reglog;
@@ -381,18 +386,17 @@ void launch_fwd_level(cb200_handle* h, const LevelPlan& P, int lv) {
             }
             g_nccl.GroupEnd();
         }
-        const int npanel = nblk(b3.maxns, WP);
-        for (int pk = 0; pk < npanel; ++pk) {
-            { FineScope fs(h, Timers::F_FWD_BIG_TRI);
-              k_big_tri_fwd<<<b3.cnt, 256, 0, h->stream>>>(ds, bl, pk, h->d_L.p, h->d_y.p);
-              LAUNCH(h); }
-            const int rows_below = b3.maxnf - pk * WP;     // upper bound
-            if (rows_below > 0) {
-                FineScope fs(h, Timers::F_FWD_BIG_GEMV);
-                k_big_gemv_fwd<<<dim3(nblk(rows_below, BRT), b3.cnt), 256, 0, h->stream>>>(
-                    ds, bl, pk, h->d_L.p, h->d_y.p, h->d_uvec.p);
-                LAUNCH(h);
-            }
+        {
+            FineScope fs(h, Timers::F_FWD_BIG_TRI);
+            unsigned* sy = h->d_bigsync.p + b3.sync_off;
+            k_big_tri_fwd<<<b3.nwork, 256, 0, h->stream>>>(ds, h->d_bigwork.p + b3.work_off, sy, sy + 2, h->d_bigsync.p,
+                                                            h->d_L.p, h->d_y.p);
+            LAUNCH(h);
+        }
+        if (b3.ntile) {
+            FineScope fs(h, Timers::F_FWD_BIG_GEMV);
+            k_big_gemv_fwd<<<b3.ntile, 256, 0, h->stream>>>(ds, h->d_bigwork.p + b3.tile_off, h->d_L.p, h->d_y.p, h->d_uvec.p);
+            LAUNCH(h);
         }
     }
     if (ms) h->join(3);
@@ -408,22 +412,18 @@ void launch_bwd_level(cb200_handle* h, const LevelPlan& P) {
     for (int pass = 0; pass < 2; ++pass) {
         const Batch& b3 = pass == 0 ? P.tops : P.solve[3];
         if (!b3.cnt) continue;
-        const int32_t* bl = h->d_batches.p + b3.off;
-        const int npanel = nblk(b3.maxns, WP);
-        const int maxtiles = std::max(1, nblk(b3.maxnf, BRT));
-        for (int pk = npanel - 1; pk >= 0; --pk) {
-            const int rows_below = b3.maxnf - pk * WP;
-            if (rows_below > 0) {
-                FineScope fs(h, Timers::F_BWD_BIG_GEMV);
-                k_big_gemvT_bwd<<<dim3(nblk(rows_below, BRT), b3.cnt), 256, 0, h->stream>>>(
-                    ds, bl, pk, maxtiles, h->d_L.p, h->d_y.p, h->d_partial.p);
-                LAUNCH(h);
-            }
-            FineScope fs(h, Timers::F_BWD_BIG_TRI);
-            k_big_tri_bwd<<<b3.cnt, 256, 0, h->stream>>>(ds, bl, pk, maxtiles, h->d_L.p, h->d_Dinv.p,
-                                                         h->d_partial.p, h->d_y.p);
+        if (b3.ntile) {
+            FineScope fs(h, Timers::F_BWD_BIG_GEMV);
+            k_big_gemvT_bwd<<<b3.ntile, 256, 0, h->stream>>>(ds, h->d_bigwork.p + b3.tile_off, h->d_L.p, h->d_y.p,
+                                                              h->d_partial.p);
             LAUNCH(h);
         }
+        FineScope fs(h, Timers::F_BWD_BIG_TRI);
+        unsigned* sy = h->d_bigsync.p + b3.sync_off;
+        k_big_tri_bwd<<<b3.nwork, 256, 0, h->stream>>>(ds, h->d_bigwork.p + b3.work_off + b3.nwork, sy + 1,
+                                                        sy + 2 + b3.nwork, h->d_bigsync.p, h->d_L.p, h->d_Dinv.p,
+                                                        h->d_partial.p, h->d_y.p);
+        LAUNCH(h);
     }
     const Batch& b2 = P.solve[2];
     if (b2.cnt) {
@@ -658,11 +658,44 @@ int build_plans(cb200_handle* h) {
         CUDA_OK(cudaStreamSynchronize(s));
     }
     CUDA_OK(h->d_W.alloc((size_t)std::max<int64_t>(1, wmax)));
-    size_t pmax = 1;
-    for (const LevelPlan& P : h->plan)
-        for (const Batch* b3 : {&P.solve[3], &P.tops})
-            if (b3->cnt) pmax = std::max(pmax, (size_t)b3->cnt * std::max(1, nblk(b3->maxnf, BRT)) * WP);
-    CUDA_OK(h->d_partial.alloc(pmax));
+    // big-solve work lists, per batch: the 64-blocks of L11 block-major across the fronts, ascending
+    // (forward) then descending (backward) - every block of a front is ticketed before the blocks that
+    // wait on it - then the 64-row tiles of L21.  d_bigsync per batch: forward ticket, backward ticket,
+    // forward flags, backward flags (one per block).
+    std::vector<BigItem> work;
+    int64_t nsync = 1, pmax = 1;
+    for (LevelPlan& P : h->plan)
+        for (Batch* b3 : {&P.solve[3], &P.tops}) {
+            if (!b3->cnt) continue;
+            std::vector<int32_t> nbk(b3->cnt), fbase(b3->cnt);
+            std::vector<int64_t> pbase(b3->cnt);
+            int32_t nflag = 0, maxnb = 0;
+            int64_t psz = 0;
+            for (int32_t k = 0; k < b3->cnt; ++k) {
+                const int32_t sn = batches[b3->off + k];
+                nbk[k] = nblk(S.ns(sn), SB); fbase[k] = nflag; nflag += nbk[k]; maxnb = std::max(maxnb, nbk[k]);
+                pbase[k] = psz; psz += (int64_t)nblk(S.nr(sn), BRT) * S.ns(sn);
+            }
+            if (psz > std::numeric_limits<int32_t>::max()) { set_error("build_plans: big-solve partial sums exceed 2^31"); return -3; }
+            b3->sync_off = nsync; nsync += 2 + 2 * (int64_t)nflag;
+            b3->work_off = (int32_t)work.size(); b3->nwork = nflag;
+            for (int dir = 0; dir < 2; ++dir)
+                for (int32_t m = 0; m < maxnb; ++m)
+                    for (int32_t k = 0; k < b3->cnt; ++k)
+                        if (m < nbk[k]) work.push_back({batches[b3->off + k], dir == 0 ? m : nbk[k] - 1 - m, fbase[k], (int32_t)pbase[k]});
+            b3->tile_off = (int32_t)work.size();
+            for (int32_t k = 0; k < b3->cnt; ++k) {
+                const int32_t sn = batches[b3->off + k];
+                for (int32_t t = 0; t * BRT < S.nr(sn); ++t)
+                    work.push_back({sn, S.ns(sn) + t * BRT, 0, (int32_t)(pbase[k] + (int64_t)t * S.ns(sn))});
+            }
+            b3->ntile = (int32_t)work.size() - b3->tile_off;
+            pmax = std::max(pmax, psz);
+        }
+    CUDA_OK(h->d_bigwork.upload(work, s));
+    CUDA_OK(h->d_bigsync.alloc((size_t)nsync));
+    CUDA_OK(h->d_partial.alloc((size_t)pmax));
+    CUDA_OK(cudaStreamSynchronize(s));
     return 0;
 }
 
@@ -879,6 +912,10 @@ size_t subtree_smem_bwd(const cb200_handle* h) { return ((size_t)h->sub_maxcols 
 
 int sweeps_body(cb200_handle* h) {
     const auto& S = h->S;
+    // tickets and ready flags of the big-solve chains start from zero in every sweep (a memset node
+    // of the captured graph); the error word [0] is reset per solve call
+    if (h->d_bigsync.n > 1)
+        CUDA_OK(cudaMemsetAsync(h->d_bigsync.p + 1, 0, (h->d_bigsync.n - 1) * sizeof(unsigned), h->stream));
     if (h->nsub) {        // the bottom subtrees first: everything above them depends on their contributions
         FineScope fs(h, Timers::F_FWD_SUB);
         k_fwd_subtree<<<h->nsub, 256, subtree_smem_fwd(h), h->stream>>>(devsym(h), subtrees(h), h->d_L.p, h->d_y.p, h->d_uvec.p);
@@ -950,6 +987,17 @@ int residual(cb200_handle* h, const double* d_xi, double* d_e, int slot) {
         LAUNCH(h);
     }
     h->tm.end(st);
+    return 0;
+}
+
+// Error word of the big-solve chains (k_big_tri_*: a ready flag not set within the spin bound), one
+// per solve call: reset before the first sweep, read back with the call's final synchronise.
+int reset_chain_error(cb200_handle* h) {
+    if (h->d_bigsync.n) CUDA_OK(cudaMemsetAsync(h->d_bigsync.p, 0, sizeof(unsigned), h->stream));
+    return 0;
+}
+int read_chain_error(cb200_handle* h, unsigned* err) {
+    if (h->d_bigsync.n) CUDA_OK(cudaMemcpyAsync(err, h->d_bigsync.p, sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
     return 0;
 }
 
@@ -1232,11 +1280,15 @@ int32_t cb200_solve(cb200_handle* h, double* x, const double* b) {
     if (N == 0) return 0;
     CUDA_OK(cudaSetDevice(h->st.device));
     CUDA_OK(cudaMemcpyAsync(h->d_b.p, b, N * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    int rc = tri_solve(h, h->d_b.p, h->d_x.p);
+    int rc = reset_chain_error(h); if (rc) return rc;
+    rc = tri_solve(h, h->d_b.p, h->d_x.p);
     if (rc) return rc;
     CUDA_OK(cudaMemcpyAsync(x, h->d_x.p, N * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    unsigned chain_err = 0;
+    rc = read_chain_error(h, &chain_err); if (rc) return rc;
     CUDA_OK(cudaStreamSynchronize(h->stream));
     h->tm.collect();
+    if (chain_err) { set_error("cb200_solve: a big-front solve chain timed out waiting for a block"); return -4; }
     return 0;
 }
 
@@ -1427,7 +1479,8 @@ int32_t cb200_solve_ir(cb200_handle* h, const double* rhsx, const double* rhsz,
     k_absmax<<<std::min(nblk(N, 256), h->reduce_blocks), 256, 0, st>>>(h->d_b.p, N, h->d_scal.p + 1);
     h->tm.nlaunch += 2;
     double* x = h->d_x.p; double* dx = h->d_dx.p; double* e = h->d_e.p;
-    int rc = tri_solve(h, h->d_b.p, x);
+    int rc = reset_chain_error(h); if (rc) return rc;
+    rc = tri_solve(h, h->d_b.p, x);
     if (rc) return rc;
     int ok = 1;
     if (h->st.iterative_refinement_enable) {
@@ -1468,8 +1521,11 @@ int32_t cb200_solve_ir(cb200_handle* h, const double* rhsx, const double* rhsz,
         if (lhsx && n) CUDA_OK(cudaMemcpyAsync(lhsx, h->d_x.p, n * sizeof(double), cudaMemcpyDeviceToHost, st));
         if (lhsz && m) CUDA_OK(cudaMemcpyAsync(lhsz, h->d_x.p + n, m * sizeof(double), cudaMemcpyDeviceToHost, st));
     }
+    unsigned chain_err = 0;
+    rc = read_chain_error(h, &chain_err); if (rc) return rc;
     CUDA_OK(cudaStreamSynchronize(st));
     h->tm.collect();
+    if (chain_err) { set_error("cb200_solve_ir: a big-front solve chain timed out waiting for a block"); ok = 0; }
     if (!ok && !h->resident) {
         // a failed solve must not leave stale finite values in the caller's vectors: the reference
         // checks all(isfinite, x) on them when refinement is disabled (kktsolver_directldl.jl:356-370)

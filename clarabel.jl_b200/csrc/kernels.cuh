@@ -1610,12 +1610,65 @@ k_bwd_cta(DevSym S, const int32_t* __restrict__ batch, const double* __restrict_
     for (int i = tid; i < ns; i += 256) y[f + i] = w[i];
 }
 
-// --- big supernodes: several CTAs per supernode.  The pivot columns are processed in panels of
-// WP columns; per panel a 1-CTA triangle kernel (inverted 64-blocks inside) and a many-CTA GEMV
-// over all rows below the panel.  The work vector lives in place: top part in y[f..f+ns), bottom
-// part in uvec[rows_ptr[s]..).  Panels run as separate launches (stream order = dependency).
-constexpr int WP = 256;        // panel width
-constexpr int BRT = 64;        // rows per CTA in the GEMV kernels
+// --- big supernodes: several CTAs per supernode, one launch per kernel and level whatever ns is.
+// The work vector lives in place: top part in y[f..f+ns), bottom part in uvec[rows_ptr[s]..).
+//   L11: one CTA per (front, 64-block).  The blocks of a front form a chain (forward: block i needs
+//        x_0..x_{i-1}; backward: block j needs x_{j+1}..); a CTA streams its strip of L while the
+//        chain advances and waits on a per-block ready flag before each product.  CTAs take their
+//        block from an atomic ticket in an order (built by build_plans) where every block of a front
+//        comes before the blocks that wait on it, so a CTA only ever waits on blocks that running
+//        CTAs hold: no deadlock, whatever the residency or the block scheduler's order.
+//   L21: 64-row tiles of every front of the level in one grid (forward: after the chain, with all of
+//        x known; backward: before it, into per-tile partial sums reduced in a fixed order).
+// Every sum runs in a fixed order, so the solves stay bitwise reproducible.
+constexpr int BRT = 64;                     // rows per CTA in the GEMV kernels
+constexpr unsigned BIG_SPIN_MAX = 1u << 22; // polls of one ready flag (~1 s) before the solve is declared failed
+
+// One item of the big-solve work lists: {supernode, 64-block (L11) or first row (L21 tile),
+// first ready flag of the front, partial-sum offset (backward L11: of the front, L21: of the tile)}.
+using BigItem = int4;
+
+__device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
+    unsigned v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_release_gpu(unsigned* p, unsigned v) {
+    asm volatile("st.release.gpu.global.u32 [%0], %1;" :: "l"(p), "r"(v) : "memory");
+}
+// x of another CTA of the same launch: a coherent (L2) load, never the non-coherent path
+__device__ __forceinline__ double ld_relaxed_gpu(const double* p) {
+    double v;
+    asm volatile("ld.relaxed.gpu.global.f64 %0, [%1];" : "=d"(v) : "l"(p));
+    return v;
+}
+
+// Block-wide: thread 0 polls `flag` (acquire) until it is set.  false (on every thread) when the
+// spin bound is exceeded or another CTA has already failed; the error word is then set.
+__device__ __forceinline__ bool big_wait(const unsigned* flag, unsigned* err) {
+    int ok = 0;
+    if (threadIdx.x == 0) {
+        for (unsigned it = 0; it < BIG_SPIN_MAX; ++it) {
+            if (ld_acquire_gpu(flag)) { ok = 1; break; }
+            if (*(volatile unsigned*)err) break;
+            __nanosleep(64);
+        }
+        if (!ok) atomicOr(err, 1u);
+    }
+    return __syncthreads_or(ok);
+}
+
+// Block-wide, after the caller's writes are visible block-wide (a preceding __syncthreads): publish.
+__device__ __forceinline__ void big_publish(unsigned* flag) {
+    if (threadIdx.x == 0) { __threadfence(); st_release_gpu(flag, 1u); }
+}
+
+__device__ __forceinline__ int big_ticket(unsigned* ticket) {
+    __shared__ int t;
+    if (threadIdx.x == 0) t = (int)atomicAdd(ticket, 1u);
+    __syncthreads();
+    return t;
+}
 
 // w = [y_s ; 0] + sum of children contributions (destination-owner form).
 // AL lanes cooperate on one destination row: AL = 1 (thread per row), 32 (warp per row: fronts with
@@ -1676,139 +1729,139 @@ k_big_asm_fwd(DevSym S, const int32_t* __restrict__ batch, double* __restrict__ 
     }
 }
 
-// forward triangle of panel pk: x = inv-blocked solve of L11[kb:kb+wp, kb:kb+wp]; grid (cnt)
+// forward, L11: one CTA per (front, 64-block i); grid = the level's blocks, order from `ticket`.
+// t = w_i - sum_{j<i} L[i,j] x_j (ascending j, each after flag j) ; x_i = inv(L_ii) t -> y ; flag i.
+// 256 threads = 64 rows x 4 column quarters; the L loads of block j+1 are in flight while the CTA
+// waits for x_j, so a hop of the chain costs a flag hand-off, not an HBM round trip.
 __global__ void __launch_bounds__(256)
-k_big_tri_fwd(DevSym S, const int32_t* __restrict__ batch, int pk, const double* __restrict__ Lst,
-              double* __restrict__ y) {
-    __shared__ double w[WP];
-    __shared__ double xs[SB];
+k_big_tri_fwd(DevSym S, const BigItem* __restrict__ work, unsigned* ticket, unsigned* flags, unsigned* err,
+              const double* __restrict__ Lst, double* y) {
+    __shared__ double ts[SB];
     __shared__ double part[4][SB];
-    const int s = batch[blockIdx.x];
+    const BigItem it = work[big_ticket(ticket)];
+    const int s = it.x, bi = it.y;
+    flags += it.z;
     const int f = S.sn_first[s];
     const int ns = S.sn_first[s + 1] - f;
-    const int kb0 = pk * WP;
-    if (kb0 >= ns) return;
-    const int wp = min(WP, ns - kb0);
-    const int nf = ns + (int)(S.rows_ptr[s + 1] - S.rows_ptr[s]);
     const int ld = S.ld[s];
-    const int tid = threadIdx.x;
-    if (tid < wp) w[tid] = y[f + kb0 + tid];
-    __syncthreads();
     const double* Lp = Lst + S.panel_off[s];
-    for (int kk = 0; kk < wp; kk += SB) {
-        const int kb = kb0 + kk;
-        const int sb = min(SB, wp - kk);
-        // the row of the panel below this block that the thread will update: its loads do not depend
-        // on x_kb, so they are issued BEFORE the block solve (one memory latency per block, not three)
-        const int r = kk + sb + tid;
-        const bool has_r = r < wp;
-        const double* rowp = Lp + (int64_t)kb * ld + kb0 + r;
-        double v[SB];
+    const int kb = bi * SB, sb = min(SB, ns - kb);
+    const int tid = threadIdx.x, r = tid & (SB - 1), q = tid >> 6;
+    const bool has_r = r < sb;
+    // row r of the inverted diagonal block, columns q, q+4, .. < r
+    double vd[16];
 #pragma unroll
-        for (int u = 0; u < SB; ++u) v[u] = (has_r && u < sb) ? rowp[(int64_t)u * ld] : 0.0;
-        {
-            const int i = tid & 63, qd = tid >> 6;
-            double acc = 0.0;
-            if (i < sb) acc = diag_row_dot(Lp + (int64_t)kb * ld + kb + i, ld, i, qd, w + kk);
-            part[qd][i] = acc;
-        }
-        __syncthreads();
-        if (tid < sb) xs[tid] = w[kk + tid] + part[0][tid] + part[1][tid] + part[2][tid] + part[3][tid];
-        __syncthreads();
-        if (tid < sb) w[kk + tid] = xs[tid];
-        if (has_r) {
-            double a0 = 0.0, a1 = 0.0;
+    for (int u = 0; u < 16; ++u) { const int j = q + 4 * u; vd[u] = (has_r && j < r) ? Lp[(int64_t)(kb + j) * ld + kb + r] : 0.0; }
+    const double wr = (tid < sb) ? y[f + kb + tid] : 0.0;      // own rows: written by earlier launches only
+    // row r of the strip left of the block, columns jb*64 + q*16 + u
+    const double* rowp = Lp + (int64_t)(q * 16) * ld + kb + r;
+    double v[16];
 #pragma unroll
-            for (int u = 0; u < SB; u += 2) { a0 += v[u] * xs[u]; a1 += v[u + 1] * xs[u + 1]; }
-            w[r] -= a0 + a1;
-        }
-        __syncthreads();
+    for (int u = 0; u < 16; ++u) v[u] = (bi > 0 && has_r) ? rowp[(int64_t)u * ld] : 0.0;
+    double a0 = 0.0, a1 = 0.0;
+    for (int jb = 0; jb < bi; ++jb) {
+        double vn[16];
+        const bool more = jb + 1 < bi && has_r;
+#pragma unroll
+        for (int u = 0; u < 16; ++u) vn[u] = more ? rowp[(int64_t)((jb + 1) * SB + u) * ld] : 0.0;
+        if (!big_wait(flags + jb, err)) return;
+        const double* xj = y + f + jb * SB + q * 16;          // a full block: only the last one is partial
+        double xv[16];
+#pragma unroll
+        for (int u = 0; u < 16; ++u) xv[u] = ld_relaxed_gpu(xj + u);
+#pragma unroll
+        for (int u = 0; u < 16; u += 2) { a0 += v[u] * xv[u]; a1 += v[u + 1] * xv[u + 1]; }
+#pragma unroll
+        for (int u = 0; u < 16; ++u) v[u] = vn[u];
     }
-    if (tid < wp) y[f + kb0 + tid] = w[tid];
+    part[q][r] = a0 + a1;
+    __syncthreads();
+    if (tid < sb) ts[tid] = wr - ((part[0][tid] + part[1][tid]) + (part[2][tid] + part[3][tid]));
+    __syncthreads();
+    {   // x_r = t_r + sum_{j<r} Linv[r,j] t_j
+        double acc = 0.0;
+#pragma unroll
+        for (int u = 0; u < 16; ++u) { const int j = q + 4 * u; if (has_r && j < r) acc += vd[u] * ts[j]; }
+        part[q][r] = acc;
+    }
+    __syncthreads();
+    if (tid < sb) y[f + kb + tid] = ts[tid] + ((part[0][tid] + part[1][tid]) + (part[2][tid] + part[3][tid]));
+    __syncthreads();
+    big_publish(flags + bi);
 }
 
-// forward GEMV below panel pk: w[r] -= sum_j L[r, kb0+j] x_j ; grid (row tiles of BRT rows, cnt).
-// 256 threads = 64 rows x 4 column quarters: short dependent chains, many CTAs even when a level
-// holds a single big front.
+// forward, L21: w[r] -= sum_{j<ns} L[r, j] x_j for the rows r >= ns of one 64-row tile; grid = the
+// level's tiles.  256 threads = 64 rows x 4 column quarters of 256-column chunks of x.
 __global__ void __launch_bounds__(256)
-k_big_gemv_fwd(DevSym S, const int32_t* __restrict__ batch, int pk, const double* __restrict__ Lst,
-               double* __restrict__ y, double* __restrict__ uvec) {
-    __shared__ double xs[WP];
+k_big_gemv_fwd(DevSym S, const BigItem* __restrict__ tiles, const double* __restrict__ Lst,
+               const double* __restrict__ y, double* __restrict__ uvec) {
+    constexpr int XC = 256;
+    __shared__ double xs[XC];
     __shared__ double red[4][BRT];
-    const int s = batch[blockIdx.y];
+    const BigItem it = tiles[blockIdx.x];
+    const int s = it.x, r0 = it.y;
     const int f = S.sn_first[s];
     const int ns = S.sn_first[s + 1] - f;
-    const int kb0 = pk * WP;
-    if (kb0 >= ns) return;
-    const int wp = min(WP, ns - kb0);
     const int64_t rp = S.rows_ptr[s];
     const int nf = ns + (int)(S.rows_ptr[s + 1] - rp);
     const int ld = S.ld[s];
-    const int r0 = kb0 + wp + blockIdx.x * BRT;
-    if (r0 >= nf) return;
     const int tid = threadIdx.x;
-    for (int j = tid; j < wp; j += 256) xs[j] = y[f + kb0 + j];
-    __syncthreads();
     const int rl = tid & (BRT - 1), q = tid / BRT;          // row in tile, column quarter
     const int r = r0 + rl;
-    double acc = 0.0;
-    if (r < nf) {
-        const double* rowp = Lst + S.panel_off[s] + (int64_t)kb0 * ld + r;
-        const int j0 = q * (WP / 4), j1 = min(wp, j0 + WP / 4);
-        double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;
-        int j = j0;
-        for (; j + 16 <= j1; j += 16) {        // (batches of 32 were measured slower: 246 registers)
-            double v[16];
+    const double* rowp = Lst + S.panel_off[s] + r;
+    double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;
+    for (int c0 = 0; c0 < ns; c0 += XC) {
+        const int cw = min(XC, ns - c0);
+        __syncthreads();                                     // the previous chunk has been consumed
+        for (int j = tid; j < cw; j += 256) xs[j] = y[f + c0 + j];
+        __syncthreads();
+        if (r < nf) {
+            const int j0 = q * (XC / 4), j1 = min(cw, j0 + XC / 4);
+            int j = j0;
+            for (; j + 16 <= j1; j += 16) {        // (batches of 32 were measured slower: 246 registers)
+                double v[16];
 #pragma unroll
-            for (int u = 0; u < 16; ++u) v[u] = rowp[(int64_t)(j + u) * ld];
+                for (int u = 0; u < 16; ++u) v[u] = rowp[(int64_t)(c0 + j + u) * ld];
 #pragma unroll
-            for (int u = 0; u < 16; u += 4) {
-                a0 += v[u] * xs[j + u]; a1 += v[u + 1] * xs[j + u + 1];
-                a2 += v[u + 2] * xs[j + u + 2]; a3 += v[u + 3] * xs[j + u + 3];
+                for (int u = 0; u < 16; u += 4) {
+                    a0 += v[u] * xs[j + u]; a1 += v[u + 1] * xs[j + u + 1];
+                    a2 += v[u + 2] * xs[j + u + 2]; a3 += v[u + 3] * xs[j + u + 3];
+                }
             }
+            for (; j < j1; ++j) a0 += rowp[(int64_t)(c0 + j) * ld] * xs[j];
         }
-        for (; j < j1; ++j) a0 += rowp[(int64_t)j * ld] * xs[j];
-        acc = (a0 + a1) + (a2 + a3);
     }
-    red[q][rl] = acc;
+    red[q][rl] = (a0 + a1) + (a2 + a3);
     __syncthreads();
-    if (q == 0 && r < nf) {
-        const double t = (red[0][rl] + red[1][rl]) + (red[2][rl] + red[3][rl]);
-        if (r < ns) y[f + r] -= t; else uvec[rp + r - ns] -= t;
-    }
+    if (q == 0 && r < nf) uvec[rp + r - ns] -= (red[0][rl] + red[1][rl]) + (red[2][rl] + red[3][rl]);
 }
 
-// backward, transposed GEMV below panel pk: partial[tile][j] = sum_{r in tile} L[r, kb0+j] w_r
-// with w_r = y[f+r] (r < ns, already solved) or y[rows[r-ns]]; grid (row tiles, cnt)
+// backward, L21: partial[tile][j] = sum_{r in tile} L[r, j] w_r for every pivot column j, with
+// w_r = y[rows[r-ns]] (ancestors, solved by earlier launches); grid = the level's tiles
 __global__ void __launch_bounds__(256)
-k_big_gemvT_bwd(DevSym S, const int32_t* __restrict__ batch, int pk, int maxtiles,
-                const double* __restrict__ Lst, const double* __restrict__ y,
-                double* __restrict__ partial) {
+k_big_gemvT_bwd(DevSym S, const BigItem* __restrict__ tiles, const double* __restrict__ Lst,
+                const double* __restrict__ y, double* __restrict__ partial) {
     __shared__ double ws[BRT];
     __shared__ double red4[8][4 * 33];
-    const int s = batch[blockIdx.y];
+    const BigItem it = tiles[blockIdx.x];
+    const int s = it.x, r0 = it.y;
     const int f = S.sn_first[s];
     const int ns = S.sn_first[s + 1] - f;
-    const int kb0 = pk * WP;
-    if (kb0 >= ns) return;
-    const int wp = min(WP, ns - kb0);
     const int64_t rp = S.rows_ptr[s];
     const int nf = ns + (int)(S.rows_ptr[s + 1] - rp);
     const int ld = S.ld[s];
-    const int r0 = kb0 + wp + blockIdx.x * BRT;
-    if (r0 >= nf) return;
     const int nrow = min(BRT, nf - r0);
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    if (tid < nrow) { const int r = r0 + tid; ws[tid] = r < ns ? y[f + r] : y[S.rows[rp + r - ns]]; }
+    if (tid < nrow) ws[tid] = y[S.rows[rp + r0 + tid - ns]];
     __syncthreads();
-    double* out = partial + ((int64_t)blockIdx.y * maxtiles + blockIdx.x) * WP;
-    const double* Lp = Lst + S.panel_off[s] + (int64_t)kb0 * ld + r0;
-    for (int j = wid * 4; j < wp; j += 32) {          // 8 warps x 4 columns per pass
+    double* out = partial + it.w;
+    const double* Lp = Lst + S.panel_off[s] + r0;
+    for (int j = wid * 4; j < ns; j += 32) {          // 8 warps x 4 columns per pass
         double a[4] = {0.0, 0.0, 0.0, 0.0};
         for (int i = lane; i < nrow; i += 32) {
             const double wv = ws[i];
 #pragma unroll
-            for (int u = 0; u < 4; ++u) if (j + u < wp) a[u] += Lp[(int64_t)(j + u) * ld + i] * wv;
+            for (int u = 0; u < 4; ++u) if (j + u < ns) a[u] += Lp[(int64_t)(j + u) * ld + i] * wv;
         }
         // cross-lane sums through shared memory (shuffles in this loop would be WARPSYNC.COLLECTIVE'd)
 #pragma unroll
@@ -1818,74 +1871,93 @@ k_big_gemvT_bwd(DevSym S, const int32_t* __restrict__ batch, int pk, int maxtile
             double v = 0.0;
 #pragma unroll
             for (int l = 0; l < 32; ++l) v += red4[wid][lane * 33 + l];
-            if (j + lane < wp) out[j + lane] = v;
+            if (j + lane < ns) out[j + lane] = v;
         }
         __syncwarp();
     }
 }
 
-// backward triangle of panel pk: t = D^-1 y_panel - sum_tiles partial ; x = L11_panel^-T t ; grid (cnt)
+// sum over the 64 rows r of a[u] held by thread (r = tid & 63, q = tid >> 6) for column q*16+u, in a
+// fixed order; thread c < 64 returns the sum of column c.  Ends with the shared tiles free again.
+__device__ __forceinline__ double big_colsum(const double (&a)[16], double (*red)[SB + 1], double (*red2)[SB]) {
+    const int tid = threadIdx.x, r = tid & (SB - 1), q = tid >> 6;
+#pragma unroll
+    for (int u = 0; u < 16; ++u) red[q * 16 + u][r] = a[u];
+    __syncthreads();
+    double s = 0.0;
+#pragma unroll
+    for (int k = 0; k < 16; ++k) s += red[r][q * 16 + k];   // column r, rows q*16..q*16+15
+    red2[q][r] = s;
+    __syncthreads();
+    const double t = tid < SB ? (red2[0][tid] + red2[1][tid]) + (red2[2][tid] + red2[3][tid]) : 0.0;
+    __syncthreads();
+    return t;
+}
+
+// backward, L11: one CTA per (front, 64-column block j); grid = the level's blocks, descending j per
+// front by the ticket order.  t = D^-1 y_j - sum_tiles partial (tile order) - sum_{i>j} L[i,j]' x_i
+// (descending i, each after flag i) ; x_j = inv(L_jj)' t -> y ; flag j.
+// 256 threads = 64 rows (of block i) x 4 column quarters; a thread needs only its own x_i entry.
 __global__ void __launch_bounds__(256)
-k_big_tri_bwd(DevSym S, const int32_t* __restrict__ batch, int pk, int maxtiles,
+k_big_tri_bwd(DevSym S, const BigItem* __restrict__ work, unsigned* ticket, unsigned* flags, unsigned* err,
               const double* __restrict__ Lst, const double* __restrict__ Dinv,
-              const double* __restrict__ partial, double* __restrict__ y) {
-    __shared__ double w[WP];
+              const double* __restrict__ partial, double* y) {
+    __shared__ double red[SB][SB + 1];
+    __shared__ double red2[4][SB];
     __shared__ double ts[SB];
-    __shared__ double red8[8][8 * 33];
-    const int s = batch[blockIdx.x];
+    const BigItem it = work[big_ticket(ticket)];
+    const int s = it.x, bj = it.y;
+    flags += it.z;
     const int f = S.sn_first[s];
     const int ns = S.sn_first[s + 1] - f;
-    const int kb0 = pk * WP;
-    if (kb0 >= ns) return;
-    const int wp = min(WP, ns - kb0);
     const int nf = ns + (int)(S.rows_ptr[s + 1] - S.rows_ptr[s]);
     const int ld = S.ld[s];
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int ntiles = (nf - kb0 - wp + BRT - 1) / BRT;
-    if (tid < wp) {
-        double acc = y[f + kb0 + tid] * Dinv[f + kb0 + tid];
-        const double* pp = partial + (int64_t)blockIdx.x * maxtiles * WP + tid;
-        for (int t = 0; t < ntiles; ++t) acc -= pp[(int64_t)t * WP];
-        w[tid] = acc;
-    }
-    __syncthreads();
     const double* Lp = Lst + S.panel_off[s];
-    const int nsub = (wp + SB - 1) / SB;
-    for (int bi = nsub - 1; bi >= 0; --bi) {
-        const int kk = bi * SB;
-        const int kb = kb0 + kk;
-        const int sb = min(SB, wp - kk);
-        {
-            const int j0 = wid * 8;
-            if (j0 < sb) {
-                const double o = cols8_dot(Lp + (int64_t)(kb + j0) * ld + kb0, ld, min(8, sb - j0), kk + sb, wp, w, lane, red8[wid]);
-                if (lane < 8 && j0 + lane < sb) ts[j0 + lane] = w[kk + j0 + lane] - o;
-            }
-        }
-        __syncthreads();
-        {
-            const int j0 = wid * 8;
-            if (j0 < sb) {
-                double a[8];
+    const int nb = (ns + SB - 1) / SB;
+    const int kb = bj * SB, sb = min(SB, ns - kb);
+    const int tid = threadIdx.x, r = tid & (SB - 1), q = tid >> 6;
+    // column q*16+u of this block in block row bi (rows bi*64 + r); for bi = bj the inverted diagonal
+    // block (row r > column).  The diagonal block comes last: it is fetched while the last wait runs.
+    const double* colp = Lp + (int64_t)(kb + q * 16) * ld + r;
+    auto fetch = [&](int bi, double (&v)[16]) {
 #pragma unroll
-                for (int u = 0; u < 8; ++u) {
-                    const int j = j0 + u;
-                    double v0 = 0.0, v1 = 0.0;
-                    if (j < sb) {
-                        const double* cj = Lp + (int64_t)(kb + j) * ld + kb;
-                        const int i0 = lane, i1 = lane + 32;
-                        if (i0 > j && i0 < sb) v0 = cj[i0] * ts[i0];
-                        if (i1 > j && i1 < sb) v1 = cj[i1] * ts[i1];
-                    }
-                    a[u] = v0 + v1;
-                }
-                const double v = warp_sum8_smem(a, red8[wid], lane);
-                if (lane < 8 && j0 + lane < sb) w[kk + j0 + lane] = ts[j0 + lane] + v;
-            }
-        }
-        __syncthreads();
+        for (int u = 0; u < 16; ++u)
+            v[u] = (bi == bj ? (r < sb && r > q * 16 + u) : bi * SB + r < ns) ? colp[(int64_t)u * ld + bi * SB] : 0.0;
+    };
+    // ... D^-1 y_j minus the L21 partial sums of the tiles, in tile order
+    double t0 = 0.0;
+    if (tid < sb) {
+        t0 = y[f + kb + tid] * Dinv[f + kb + tid];
+        const double* pp = partial + it.w + kb + tid;
+        const int ntiles = (nf - ns + BRT - 1) / BRT;
+        for (int t = 0; t < ntiles; ++t) t0 -= pp[(int64_t)t * ns];
     }
-    if (tid < wp) y[f + kb0 + tid] = w[tid];
+    // ... and the blocks i > j below it
+    double acc[16], v[16];
+#pragma unroll
+    for (int u = 0; u < 16; ++u) acc[u] = 0.0;
+    fetch(nb - 1, v);
+    for (int bi = nb - 1; bi > bj; --bi) {
+        double vn[16];
+        fetch(bi - 1, vn);
+        if (!big_wait(flags + bi, err)) return;
+        const int ri = bi * SB + r;
+        const double xr = ri < ns ? ld_relaxed_gpu(y + f + ri) : 0.0;
+#pragma unroll
+        for (int u = 0; u < 16; ++u) { acc[u] += v[u] * xr; v[u] = vn[u]; }
+    }
+    const double o = big_colsum(acc, red, red2);
+    if (tid < sb) ts[tid] = t0 - o;
+    __syncthreads();
+    {   // x_c = t_c + sum_{r>c} Linv[r,c] t_r
+        const double tr = r < sb ? ts[r] : 0.0;
+#pragma unroll
+        for (int u = 0; u < 16; ++u) acc[u] = v[u] * tr;      // v: the diagonal block
+    }
+    const double c = big_colsum(acc, red, red2);
+    if (tid < sb) y[f + kb + tid] = ts[tid] + c;
+    __syncthreads();
+    big_publish(flags + bj);
 }
 
 // ------------------------------------------------------------------ G8 residual e = b - K x
