@@ -60,6 +60,7 @@ template <class T> struct DevBuf {
 };
 
 struct Batch { int32_t off = 0, cnt = 0, maxnf = 0, maxns = 0, maxnr = 0, maxpanel = 0; bool many_children = false;
+               bool pre_assembled = false;    // large: some front has more than MANY_CHILDREN children (k_assemble_atomic)
                int32_t schur_t128 = 0, schur_t64 = 0;
                int32_t src_per_row = 0;
                // big solve class: the 64-blocks of L11 (forward ticket order, then backward) and the 64-row
@@ -550,6 +551,7 @@ int build_plans(cb200_handle* h) {
             b.maxnr = std::max(b.maxnr, S.nr(sn));
             b.maxpanel = std::max(b.maxpanel, nf * S.ns(sn) + 25 * nf);      // smem need of k_factor_panel
             if (S.child_ptr[sn + 1] - S.child_ptr[sn] > 64) b.many_children = true;
+            if (S.child_ptr[sn + 1] - S.child_ptr[sn] > MANY_CHILDREN) b.pre_assembled = true;
             b.src_per_row = std::max<int32_t>(b.src_per_row, (int32_t)((S.asm_base[sn + 1] - S.asm_base[sn]) / std::max(1, nf)));
             if (large && !h->to_large(nf, S.ns(sn))) b.all_padded = false;   // multi-GPU: small top fronts on the large path
             if (large && S.nr(sn) > 0) {
@@ -717,9 +719,10 @@ int allreduce_fronts(cb200_handle* h, const Batch& B, const std::vector<int32_t>
     return 0;
 }
 
-// zero the update blocks of the large fronts of one level
-__global__ void k_zero_upd(DevSym S, const int32_t* batch, double* Ust) {
+// zero the update blocks of the pre-assembled large fronts of one level (kernels.cuh, G6)
+__global__ void k_zero_upd(DevSym S, const int32_t* batch, int gather, double* Ust) {
     const int s = batch[blockIdx.y];
+    if (gathers_update(S, s, gather)) return;
     const int64_t nr = S.rows_ptr[s + 1] - S.rows_ptr[s];
     double* U = Ust + S.upd_off[s];
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < nr * nr;
@@ -813,12 +816,16 @@ int factor_body(cb200_handle* h, bool static_reg) {
             const bool is_top = pass == 1;
             const int32_t* bl = h->d_batches.p + B.off;
             const int64_t* wo = h->d_woff.p + B.off;
+            // the update blocks of the replicated top fronts are summed over the GPUs before their Schur
+            // update, so they are pre-assembled; other fronts gather theirs in the Schur epilogue
+            const int gather = is_top ? 0 : 1;
             if (h->detail) h->tm.begin(Timers::ASM, st);
-            { FineScope fs(h, Timers::F_ZERO);
-              k_zero_upd<<<dim3(std::max(1, std::min(64, nblk((int64_t)B.maxnr * B.maxnr, 1024))), B.cnt), 256, 0, st>>>(ds, bl, h->d_U.p);
+            if (!gather || B.pre_assembled) {
+              FineScope fs(h, Timers::F_ZERO);
+              k_zero_upd<<<dim3(std::max(1, std::min(64, nblk((int64_t)B.maxnr * B.maxnr, 1024))), B.cnt), 256, 0, st>>>(ds, bl, gather, h->d_U.p);
               LAUNCH(h); }
             { FineScope fs(h, Timers::F_ASM);
-              k_assemble_large<<<dim3(nblk(B.maxnf, ASM_CW), B.cnt), 256, 0, st>>>(ds, bl, h->d_L.p, h->d_U.p);
+              k_assemble_large<<<dim3(nblk(gather ? B.maxns : B.maxnf, ASM_CW), B.cnt), 256, 0, st>>>(ds, bl, gather, h->d_L.p, h->d_U.p);
               LAUNCH(h);
               for (int32_t k = 0; k < B.cnt; ++k) {
                   const int32_t sn = h->h_batches[B.off + k];
@@ -853,16 +860,14 @@ int factor_body(cb200_handle* h, bool static_reg) {
                 }
                 const int ny = mode == 0 ? B.active(J0 + PB) : B.cnt;     // fronts that still have panel columns to update
                 if (ny <= 0) return;
-                static const int dbg_fence = getenv("CB200_TMA_FENCE") ? 2 : 0;                       // debugging aids
-                static const size_t dbg_pad = getenv("CB200_TMA_PAD_KB") ? (size_t)atoi(getenv("CB200_TMA_PAD_KB")) * 1024 : 0;
                 if (tma && T == 128)
                     k_ldl_update_tma<128><<<dim3(gx, ny), tma_threads(128), tma_gemm_smem(128), st>>>(
-                        ds, bl, h->d_tmaps.p, h->d_tmap_of.p, mode, J0, na, h->tma_kmajor | dbg_fence, h->d_L.p, h->d_U.p, h->d_D.p);
+                        ds, bl, h->d_tmaps.p, h->d_tmap_of.p, mode, J0, na, gather, h->tma_kmajor, h->d_L.p, h->d_U.p, h->d_D.p);
                 else if (tma)
-                    k_ldl_update_tma<64><<<dim3(gx, ny), tma_threads(64), tma_gemm_smem(64) + dbg_pad, st>>>(
-                        ds, bl, h->d_tmaps64.p, h->d_tmap_of.p, mode, J0, na, h->tma_kmajor | dbg_fence, h->d_L.p, h->d_U.p, h->d_D.p);
+                    k_ldl_update_tma<64><<<dim3(gx, ny), tma_threads(64), tma_gemm_smem(64), st>>>(
+                        ds, bl, h->d_tmaps64.p, h->d_tmap_of.p, mode, J0, na, gather, h->tma_kmajor, h->d_L.p, h->d_U.p, h->d_D.p);
                 else
-                    k_ldl_update_ldg<<<dim3(gx, ny), 256, 0, st>>>(ds, bl, mode, J0, na, h->d_L.p, h->d_U.p, h->d_D.p);
+                    k_ldl_update_ldg<<<dim3(gx, ny), 256, 0, st>>>(ds, bl, mode, J0, na, gather, h->d_L.p, h->d_U.p, h->d_D.p);
                 LAUNCH(h);
             };
             for (int kb = 0; kb < B.maxns; kb += PB) {
@@ -1159,11 +1164,7 @@ int32_t cb200_create(int64_t N, const int64_t* colptr, const int64_t* rowval, co
         CUDA_OK(cudaFuncSetAttribute(k_piv_rows, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (2 * PB * (PB + 1)) * (int)sizeof(double)));
         CUDA_OK(cudaFuncSetAttribute(k_ldl_update_tma<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tma_gemm_smem(128)));
-        {   // (CB200_TMA_ATTR_KB: debugging aid, see DESIGN.md section 8 "reproducibility")
-            const char* e = getenv("CB200_TMA_ATTR_KB");
-            const int attr = e ? atoi(e) * 1024 + 64 : 200 * 1024;
-            CUDA_OK(cudaFuncSetAttribute(k_ldl_update_tma<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, attr));
-        }
+        CUDA_OK(cudaFuncSetAttribute(k_ldl_update_tma<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tma_gemm_smem(64)));
         { int rct = build_tensor_maps(h); if (rct) return rct; }
         CUDA_OK(cudaFuncSetAttribute(k_fwd_subtree, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
         CUDA_OK(cudaFuncSetAttribute(k_bwd_subtree, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));

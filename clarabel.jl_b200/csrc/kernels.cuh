@@ -7,7 +7,8 @@
 //   G4  small-front LDL' (shared memory)  k_factor_small (nf <= 64), k_factor_panel (64 < nf <= 152)
 //   G5  large-front blocked LDL'          k_piv_diag, k_piv_rows, k_ldl_update_tma (TMA-fed 128 x 128 DMMA GEMM),
 //                                         k_ldl_update_ldg (fallback), k_finish_large
-//   G6  extend-add                        fused in G4 ; k_assemble_large ; k_assemble_atomic
+//   G6  extend-add                        fused in G4 ; k_assemble_large ; gather_update_tile (Schur epilogue) ;
+//                                         k_assemble_atomic
 //   G7  multifrontal triangular solves    k_fwd_{leaf,warp<16|32>,cta}, k_bwd_*, k_big_{asm,tri,gemv}_*, k_*_subtree,
 //                                         k_pack_perm, k_unpack_perm
 //   G8  symmetric SpMV residual + norm    k_residual, k_residual_long
@@ -352,11 +353,22 @@ k_factor_panel(DevSym S, const int32_t* __restrict__ batch, int maxpanel, int ma
 }
 
 // ------------------------------------------------------------------ G6 assembly for large fronts
-// grid (ceil(maxnf / 8), nbatch), 256 threads: one warp per destination column of the front;
-// sources ordered by child (deterministic), no inter-warp conflicts, no barriers.
+// Large fronts come in two kinds.  A gather front (the default: at most MANY_CHILDREN children, not a
+// replicated top front) has only its panel columns assembled here; its update block U is never zeroed
+// or pre-assembled: the Schur epilogue builds each tile of U from the children (gather_update_tile)
+// and writes U = sum - L21 D L21' once.  A pre-assembled front (more than MANY_CHILDREN children:
+// k_assemble_atomic; multi-GPU top fronts: summed by NCCL before the Schur GEMM) is zeroed
+// (k_zero_upd), fully assembled and then updated in place by the epilogue.
+__device__ __forceinline__ bool gathers_update(const DevSym& S, int s, int gather) {
+    return gather && S.child_ptr[s + 1] - S.child_ptr[s] <= MANY_CHILDREN;
+}
+
+// grid (ceil(maxnf / 8), nbatch) (ceil(maxns / 8) for a gather batch), 256 threads: one warp per
+// destination column of the front; sources ordered by child (deterministic), no inter-warp
+// conflicts, no barriers.
 constexpr int ASM_CW = 8;
 __global__ void __launch_bounds__(256)
-k_assemble_large(DevSym S, const int32_t* __restrict__ batch, double* __restrict__ Lst,
+k_assemble_large(DevSym S, const int32_t* __restrict__ batch, int gather, double* __restrict__ Lst,
                  double* __restrict__ Ust) {
     const int s = batch[blockIdx.y];
     const int f = S.sn_first[s];
@@ -366,7 +378,7 @@ k_assemble_large(DevSym S, const int32_t* __restrict__ batch, double* __restrict
     const int ld = S.ld[s];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const int d = blockIdx.x * ASM_CW + wid;
-    if (d >= nf) return;
+    if (d >= (gather ? ns : nf)) return;
     if (S.child_ptr[s + 1] - S.child_ptr[s] > MANY_CHILDREN) return;     // k_assemble_atomic
     double* Lp = Lst + S.panel_off[s];
     double* Us = Ust + S.upd_off[s];
@@ -483,6 +495,60 @@ __device__ __forceinline__ UpdTile decode_update_tile(int mode, int J0, int na, 
     return u;
 }
 
+// Entry (row r, column c) of a T x T column-major tile in shared memory.  The XOR moves the four
+// column pairs of one accumulator fragment onto different banks.
+template <int T>
+__device__ __forceinline__ int tile_idx(int r, int c) { return c * T + (r ^ (((c >> 1) & 3) << 3)); }
+
+// Schur epilogue of a gather front: builds the tile (rows r0.., columns c0..) of the sum of the
+// children's contributions to U in shared memory, in the order of k_assemble_large (every entry is
+// 0 + c1 + c2 + ... over the sources of its column in child order), so that U = tile - acc is
+// bitwise what assembling U first and updating it in place gives.  Warp w of the nthr / 32 walks the
+// front columns c0 + w, c0 + w + nthr / 32, ...  The child rows of a source that land in the row
+// window start at the lower bound of r0 in the child's ascending rel; the bound does not depend on
+// the column, so each warp keeps the last child's.  sync() synchronises the nthr threads; the first
+// one lets the tile alias buffers the threads were still reading.
+template <int T, class Sync>
+__device__ __forceinline__ void gather_update_tile(const DevSym& S, int s, int ns, int nf,
+                                                   const double* __restrict__ Ust, int r0, int c0,
+                                                   double* tile, int tid, int nthr, Sync sync) {
+    sync();
+    for (int e = tid; e < T * T; e += nthr) tile[e] = 0.0;
+    sync();
+    const int lane = tid & 31;
+    const int32_t* cp = S.asm_colptr + S.front_ptr[s];
+    const int64_t base = S.asm_base[s];
+    int cc = -1, clb = 0;                          // child whose lower bound of r0 is known, and the bound
+    for (int dl = tid >> 5; dl < T; dl += nthr >> 5) {
+        const int d = c0 + dl;
+        if (d < ns || d >= nf) continue;
+        for (int e = cp[d]; e < cp[d + 1]; ++e) {
+            const int c = S.asm_child[base + e];
+            if (S.active && !S.active[c]) continue;
+            const int64_t rp0 = S.rows_ptr[c];
+            const int nrc = (int)(S.rows_ptr[c + 1] - rp0);
+            const int j = (int)(S.asm_src[base + e] - rp0);
+            const int32_t* relc = S.rel + rp0;
+            int i0 = j;                            // child row j is front row d; rows below it map below d
+            if (r0 > d) {
+                if (c != cc) {
+                    int lo = j, hi = nrc;
+                    while (lo < hi) { const int m = (lo + hi) >> 1; if (relc[m] < r0) lo = m + 1; else hi = m; }
+                    cc = c; clb = lo;
+                }
+                i0 = max(j, clb);
+            }
+            const double* src = Ust + S.upd_off[c] + (int64_t)j * nrc;
+            for (int i = i0 + lane; i < nrc; i += 32) {
+                const int r = relc[i] - r0;
+                if (r >= T) break;
+                tile[tile_idx<T>(r, dl)] += src[i];
+            }
+        }
+    }
+    sync();
+}
+
 // acc (4 x 4 per thread, rows tx*4+a, cols ty*4+c) = sum_{k in [k0,k1)} L[rowA0+i, k] D[k] L[rowB0+j, k]
 // 64 x 64 tile, 256 threads = 8 warps (2 x 4), each warp 32 x 16 of the tile as 4 x 2 DMMA fragments.
 // K-step 16, register prefetch of the next K-slab, double-buffered shared memory with a 72-double
@@ -568,9 +634,10 @@ __device__ __forceinline__ void ldl_gemm_tile(const double* __restrict__ Lp, int
 }
 
 __global__ void __launch_bounds__(256)
-k_ldl_update_ldg(DevSym S, const int32_t* __restrict__ batch, int mode, int J0, int na,
+k_ldl_update_ldg(DevSym S, const int32_t* __restrict__ batch, int mode, int J0, int na, int gather,
                  double* __restrict__ Lst, double* __restrict__ Ust, const double* __restrict__ D) {
     __shared__ double gsm[GSM];
+    static_assert(GBM * GBM <= GSM, "the gathered tile aliases the operand buffers");
     const int s = batch[blockIdx.y];
     const int f = S.sn_first[s];
     const int ns = S.sn_first[s + 1] - f;
@@ -582,6 +649,9 @@ k_ldl_update_ldg(DevSym S, const int32_t* __restrict__ batch, int mode, int J0, 
     double* Lp = Lst + S.panel_off[s];
     double acc[4][4];
     ldl_gemm_tile(Lp, ld, nf, D + f, u.ti * GBM, u.tj * GBM, u.k0, u.k1, acc, gsm);
+    const bool gat = mode == 1 && gathers_update(S, s, gather);
+    if (gat) gather_update_tile<GBM>(S, s, ns, nf, Ust, u.ti * GBM, u.tj * GBM, gsm, threadIdx.x, 256,
+                                     [] { __syncthreads(); });
     double* Us = Ust + S.upd_off[s];
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
     double cv[4][4];
@@ -594,7 +664,8 @@ k_ldl_update_ldg(DevSym S, const int32_t* __restrict__ batch, int mode, int J0, 
 #pragma unroll
         for (int a = 0; a < 4; ++a) {
             const int row = u.ti * GBM + tx * 4 + a;
-            cv[a][c] = (okc && row < nf && row >= col) ? dc[c][row] : 0.0;
+            cv[a][c] = !(okc && row < nf && row >= col) ? 0.0
+                     : gat ? gsm[tile_idx<GBM>(row - u.ti * GBM, col - u.tj * GBM)] : dc[c][row];
         }
     }
 #pragma unroll
@@ -651,9 +722,10 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
 template <int T>
 __global__ void __launch_bounds__(tma_threads(T), T == 128 ? 1 : 3)
 k_ldl_update_tma(DevSym S, const int32_t* __restrict__ batch, const CUtensorMap* __restrict__ maps,
-                 const int32_t* __restrict__ map_of, int mode, int J0, int na, int kmajor,
+                 const int32_t* __restrict__ map_of, int mode, int J0, int na, int gather, int kmajor,
                  double* __restrict__ Lst, double* __restrict__ Ust, const double* __restrict__ D) {
     extern __shared__ __align__(128) unsigned char tma_smem[];
+    static_assert(T * T <= 2 * TSTAGES * T * TK, "the gathered tile aliases the stage ring");
     const int s = batch[blockIdx.y];
     const int f = S.sn_first[s];
     const int ns = S.sn_first[s + 1] - f;
@@ -752,6 +824,11 @@ k_ldl_update_tma(DevSym S, const int32_t* __restrict__ batch, const CUtensorMap*
     }
     // ===== epilogue: subtract into the panel (col < ns) or the update block.  All loads of a column
     // pair are issued before the first store (a plain  *p -= v  loop serialises 64 load->store chains).
+    // A gather front's U tile is built in the stage ring instead: every stage has been waited on, so
+    // no TMA write is in flight, and the producer warp has returned (named barrier 1, consumers only).
+    const bool gat = mode == 1 && gathers_update(S, s, gather);
+    if (gat) gather_update_tile<T>(S, s, ns, nf, Ust, u.ti * T, u.tj * T, sA, tid, NCW * 32,
+                                   [] { asm volatile("bar.sync 1, %0;\n" :: "n"(NCW * 32) : "memory"); });
     double* Lp = Lst + S.panel_off[s];
     double* Us = Ust + S.upd_off[s];
 #pragma unroll
@@ -767,7 +844,8 @@ k_ldl_update_tma(DevSym S, const int32_t* __restrict__ batch, const CUtensorMap*
 #pragma unroll
             for (int i = 0; i < 2 * MI; ++i) {
                 const int row = u.ti * T + wm + 8 * i + g;
-                cv[e][i] = (okc[e] && row < nf && row >= col) ? dc[e][row] : 0.0;
+                cv[e][i] = !(okc[e] && row < nf && row >= col) ? 0.0
+                         : gat ? sA[tile_idx<T>(row - u.ti * T, col - u.tj * T)] : dc[e][row];
             }
         }
 #pragma unroll
