@@ -61,7 +61,8 @@ template <class T> struct DevBuf {
 
 struct Batch { int32_t off = 0, cnt = 0, maxnf = 0, maxns = 0, maxnr = 0, maxpanel = 0; bool many_children = false;
                bool pre_assembled = false;    // large: some front has more than MANY_CHILDREN children (k_assemble_atomic)
-               int32_t schur_t128 = 0, schur_t64 = 0;
+               // large: the batch's slices of the Schur and assembly tile lists (build_tile_lists)
+               int32_t schur_off = 0, nschur = 0, asm_off = 0, nasm = 0;
                int32_t src_per_row = 0;
                // big solve class: the 64-blocks of L11 (forward ticket order, then backward) and the 64-row
                // tiles of L21 in d_bigwork, and the tickets + ready flags in d_bigsync (build_plans)
@@ -238,10 +239,14 @@ struct cb200_handle {
                                       // fastest on the H100, DESIGN.md section 4), 128 (1 CTA per SM, spills on sm_90a),
                                       // or 0 = by front size (CB200_TMA_TILE)
     DevBuf<CUtensorMap> d_tmaps, d_tmaps64; DevBuf<int32_t> d_tmap_of;
+    // per-tile source lists of the large fronts, all batches (build_tile_lists)
+    DevBuf<TileEntry> d_schur_tiles, d_asm_tiles; DevBuf<TileRect> d_schur_rects, d_asm_rects;
+    int64_t n_schur_tiles = 0, n_schur_rects = 0, n_asm_tiles = 0, n_asm_rects = 0;
     // multi-GPU state
     bool dist = false; int rank = 0, nranks = 1;
     ncclComm_t comm = nullptr;
     std::vector<int32_t> owner; std::vector<int8_t> is_top;
+    std::vector<int8_t> h_active;       // host copy of d_active (DevSym::active)
     std::vector<int32_t> h_top_list;
     std::vector<std::vector<int32_t>> h_top_by_level;
     DevBuf<int8_t> d_active, d_keepcol, d_topcolkeep;
@@ -554,10 +559,6 @@ int build_plans(cb200_handle* h) {
             if (S.child_ptr[sn + 1] - S.child_ptr[sn] > MANY_CHILDREN) b.pre_assembled = true;
             b.src_per_row = std::max<int32_t>(b.src_per_row, (int32_t)((S.asm_base[sn + 1] - S.asm_base[sn]) / std::max(1, nf)));
             if (large && !h->to_large(nf, S.ns(sn))) b.all_padded = false;   // multi-GPU: small top fronts on the large path
-            if (large && S.nr(sn) > 0) {
-                b.schur_t128 = std::max(b.schur_t128, (nf - 1) / TB - S.ns(sn) / TB + 1);
-                b.schur_t64 = std::max(b.schur_t64, (nf - 1) / GBM - S.ns(sn) / GBM + 1);
-            }
             batches.push_back(sn);
             woff.push_back(large ? w : 0);
             if (large) w += (int64_t)nblk(S.ns(sn), PB) * PB * PB;   // parked diagonal blocks
@@ -701,6 +702,43 @@ int build_plans(cb200_handle* h) {
     return 0;
 }
 
+// CTA tile of a large batch's GEMMs: 64 for the LDG kernel, else CB200_TMA_TILE (0: by front size)
+int gemm_tile(const cb200_handle* h, const Batch& B) {
+    if (!(h->use_tma && B.all_padded)) return GBM;
+    return h->tma_tile == 64 || h->tma_tile == 128 ? h->tma_tile : (B.maxnf >= 1024 ? 128 : 64);
+}
+
+// Schur and assembly tile lists of every large batch (the Schur list for the batch's GEMM tile), after
+// build_plans and build_tensor_maps.  They depend on the symbolic structure only.
+int upload_tile_lists(cb200_handle* h) {
+    const Symbolic& S = h->S;
+    std::vector<TileEntry> st, at; std::vector<TileRect> sr, ar;
+    // multi-GPU: the children this rank does not assemble get no rectangles (DevSym::active)
+    const int8_t* act = h->dist ? h->h_active.data() : nullptr;
+    for (LevelPlan& P : h->plan)
+        for (Batch* B : {&P.large, &P.topf}) {
+            if (!B->cnt) continue;
+            const bool gather = B == &P.large;
+            const int32_t* fr = h->h_batches.data() + B->off;
+            B->schur_off = (int32_t)st.size();
+            build_tile_lists(S, fr, B->cnt, gemm_tile(h, *B), true, gather, act, st, sr);
+            B->nschur = (int32_t)st.size() - B->schur_off;
+            B->asm_off = (int32_t)at.size();
+            build_tile_lists(S, fr, B->cnt, ASM_T, false, gather, act, at, ar);
+            B->nasm = (int32_t)at.size() - B->asm_off;
+        }
+    h->n_schur_tiles = (int64_t)st.size(); h->n_schur_rects = (int64_t)sr.size();
+    h->n_asm_tiles = (int64_t)at.size(); h->n_asm_rects = (int64_t)ar.size();
+    st.push_back({0, 0, 0, (int32_t)sr.size()}); at.push_back({0, 0, 0, (int32_t)ar.size()});
+    if (sr.empty()) sr.resize(1);
+    if (ar.empty()) ar.resize(1);
+    cudaStream_t s = h->stream;
+    CUDA_OK(h->d_schur_tiles.upload(st, s)); CUDA_OK(h->d_schur_rects.upload(sr, s));
+    CUDA_OK(h->d_asm_tiles.upload(at, s)); CUDA_OK(h->d_asm_rects.upload(ar, s));
+    CUDA_OK(cudaStreamSynchronize(s));
+    return 0;
+}
+
 // all-reduce (sum) of the panel and update block of every front of a batch, one NCCL group
 int allreduce_fronts(cb200_handle* h, const Batch& B, const std::vector<int32_t>& list) {
     const Symbolic& S = h->S;
@@ -825,8 +863,11 @@ int factor_body(cb200_handle* h, bool static_reg) {
               k_zero_upd<<<dim3(std::max(1, std::min(64, nblk((int64_t)B.maxnr * B.maxnr, 1024))), B.cnt), 256, 0, st>>>(ds, bl, gather, h->d_U.p);
               LAUNCH(h); }
             { FineScope fs(h, Timers::F_ASM);
-              k_assemble_large<<<dim3(nblk(gather ? B.maxns : B.maxnf, ASM_CW), B.cnt), 256, 0, st>>>(ds, bl, gather, h->d_L.p, h->d_U.p);
-              LAUNCH(h);
+              if (B.nasm) {
+                  k_assemble_tiles<<<B.nasm, 256, 0, st>>>(ds, bl, h->d_asm_tiles.p + B.asm_off, h->d_asm_rects.p, gather,
+                                                           h->d_L.p, h->d_U.p);
+                  LAUNCH(h);
+              }
               for (int32_t k = 0; k < B.cnt; ++k) {
                   const int32_t sn = h->h_batches[B.off + k];
                   const int32_t nch = S.child_ptr[sn + 1] - S.child_ptr[sn];
@@ -843,31 +884,33 @@ int factor_body(cb200_handle* h, bool static_reg) {
             if (h->detail) { h->tm.end(st); h->tm.begin(Timers::PANEL, st); }
             const size_t smrows = (size_t)(2 * PB * (PB + 1)) * sizeof(double);
             // one update launch (either version): mode 0 = panel step at pivot block J0, mode 1 = Schur
+            // mode 1 runs over the batch's Schur tile list, which was built for this same tile size
             auto launch_update = [&](int mode, int J0) {
                 const bool tma = h->use_tma && B.all_padded;
-                const int T = !tma ? GBM : (h->tma_tile == 64 || h->tma_tile == 128 ? h->tma_tile : (B.maxnf >= 1024 ? 128 : 64));
-                int gx, na = 1;
+                const int T = gemm_tile(h, B);
+                int gx, ny, na = 1;
+                const TileEntry* tl = nullptr;
                 if (mode == 0) {
                     const int tj0 = (J0 + PB) / T;
                     const int nbt = (B.maxns - 1) / T - tj0 + 1;          // panel column tiles still to update
                     na = (B.maxnf - 1) / T - tj0 + 1;
                     if (nbt <= 0 || na <= 0) return;
                     gx = nbt * na;
+                    ny = B.active(J0 + PB);                                // fronts that still have panel columns to update
                 } else {
-                    const int t = T == 128 ? B.schur_t128 : B.schur_t64;
-                    if (t <= 0) return;
-                    gx = t * (t + 1) / 2;
+                    gx = B.nschur; ny = 1;
+                    tl = h->d_schur_tiles.p + B.schur_off;
                 }
-                const int ny = mode == 0 ? B.active(J0 + PB) : B.cnt;     // fronts that still have panel columns to update
-                if (ny <= 0) return;
+                if (gx <= 0 || ny <= 0) return;
+                const TileRect* rc = h->d_schur_rects.p;
                 if (tma && T == 128)
                     k_ldl_update_tma<128><<<dim3(gx, ny), tma_threads(128), tma_gemm_smem(128), st>>>(
-                        ds, bl, h->d_tmaps.p, h->d_tmap_of.p, mode, J0, na, gather, h->tma_kmajor, h->d_L.p, h->d_U.p, h->d_D.p);
+                        ds, bl, tl, rc, h->d_tmaps.p, h->d_tmap_of.p, mode, J0, na, gather, h->tma_kmajor, h->d_L.p, h->d_U.p, h->d_D.p);
                 else if (tma)
                     k_ldl_update_tma<64><<<dim3(gx, ny), tma_threads(64), tma_gemm_smem(64), st>>>(
-                        ds, bl, h->d_tmaps64.p, h->d_tmap_of.p, mode, J0, na, gather, h->tma_kmajor, h->d_L.p, h->d_U.p, h->d_D.p);
+                        ds, bl, tl, rc, h->d_tmaps64.p, h->d_tmap_of.p, mode, J0, na, gather, h->tma_kmajor, h->d_L.p, h->d_U.p, h->d_D.p);
                 else
-                    k_ldl_update_ldg<<<dim3(gx, ny), 256, 0, st>>>(ds, bl, mode, J0, na, gather, h->d_L.p, h->d_U.p, h->d_D.p);
+                    k_ldl_update_ldg<<<dim3(gx, ny), 256, 0, st>>>(ds, bl, tl, rc, mode, J0, na, gather, h->d_L.p, h->d_U.p, h->d_D.p);
                 LAUNCH(h);
             };
             for (int kb = 0; kb < B.maxns; kb += PB) {
@@ -1166,6 +1209,7 @@ int32_t cb200_create(int64_t N, const int64_t* colptr, const int64_t* rowval, co
         CUDA_OK(cudaFuncSetAttribute(k_ldl_update_tma<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tma_gemm_smem(128)));
         CUDA_OK(cudaFuncSetAttribute(k_ldl_update_tma<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tma_gemm_smem(64)));
         { int rct = build_tensor_maps(h); if (rct) return rct; }
+        { int rcl = upload_tile_lists(h); if (rcl) return rcl; }
         CUDA_OK(cudaFuncSetAttribute(k_fwd_subtree, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
         CUDA_OK(cudaFuncSetAttribute(k_bwd_subtree, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
         CUDA_OK(cudaFuncSetAttribute(k_bwd_warp<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
@@ -1627,10 +1671,12 @@ int32_t cb200_dist_init(cb200_handle* h, int32_t rank, int32_t nranks, const cha
         }
         cudaStream_t s = h->stream;
         CUDA_OK(h->d_active.upload(active, s)); CUDA_OK(h->d_keepcol.upload(keep, s));
+        h->h_active = active;
         CUDA_OK(h->d_topcolkeep.upload(topkeep, s)); CUDA_OK(h->d_top_list.upload(h->h_top_list, s));
         // update blocks of supernodes other ranks own are never written here: keep them zero
         CUDA_OK(cudaMemsetAsync(h->d_U.p, 0, h->d_U.n * sizeof(double), s));
         int rc = build_plans(h);
+        if (!rc) rc = upload_tile_lists(h);
         if (rc) return rc;
         // the captured launch sequences (if any) belong to the single-GPU plans
         for (GraphExec* g : {&h->g_factor[0], &h->g_factor[1], &h->g_solve}) {
@@ -1676,12 +1722,13 @@ int32_t cb200_get_stats(const cb200_handle* h, double* out, int32_t len) {
         }
         if (nf * ns >= 65536 && ns > 32) big_bytes += 8.0 * nf * ns;
     }
-    double v[17] = {S.flops, schur, panel_large - schur, (double)S.nnzL, (double)S.nlevels, (double)S.nsuper,
+    double v[21] = {S.flops, schur, panel_large - schur, (double)S.nnzL, (double)S.nlevels, (double)S.nsuper,
                     nlarge, big_bytes, (double)S.upd_total * 8.0, (double)S.panel_off.back() * 8.0,
                     (double)S.ordering_used, my_flops, h->use_tma ? 1.0 : 0.0, (double)h->tma_kmajor,
                     (double)((h->g_factor[0].exec != nullptr) + (h->g_factor[1].exec != nullptr)),
-                    h->g_solve.exec ? 1.0 : 0.0, (double)h->nsub};
-    for (int i = 0; i < len && i < 17; ++i) out[i] = v[i];
+                    h->g_solve.exec ? 1.0 : 0.0, (double)h->nsub,
+                    (double)h->n_schur_tiles, (double)h->n_schur_rects, (double)h->n_asm_tiles, (double)h->n_asm_rects};
+    for (int i = 0; i < len && i < 21; ++i) out[i] = v[i];
     return 0;
 }
 

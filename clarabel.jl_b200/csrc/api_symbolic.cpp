@@ -136,4 +136,31 @@ int32_t cb200_symbolic_get(const cb200_symbolic* s, int32_t which, int64_t* out,
     cb200::set_error("cb200_symbolic_get: bad selector"); return -2;
 }
 
+int32_t cb200_symbolic_tile_lists(const cb200_symbolic* s, const int64_t* fronts, int32_t nfronts, int32_t T,
+                                  int32_t schur, int32_t gather, const int64_t* active, int64_t* counts,
+                                  int64_t* tiles, int64_t* rects) {
+    const auto& S = s->S;
+    if (T != 64 && T != 128) { cb200::set_error("cb200_symbolic_tile_lists: T must be 64 or 128"); return -2; }
+    std::vector<int32_t> fr(nfronts);
+    for (int32_t k = 0; k < nfronts; ++k) {
+        if (fronts[k] < 0 || fronts[k] >= S.nsuper) { cb200::set_error("cb200_symbolic_tile_lists: bad front"); return -2; }
+        fr[k] = (int32_t)fronts[k];
+    }
+    std::vector<int8_t> act;
+    if (active) { act.resize(S.nsuper); for (int32_t q = 0; q < S.nsuper; ++q) act[q] = active[q] != 0; }
+    std::vector<cb200::TileEntry> te; std::vector<cb200::TileRect> tr;
+    cb200::build_tile_lists(S, fr.data(), nfronts, T, schur != 0, gather != 0, active ? act.data() : nullptr, te, tr);
+    counts[0] = (int64_t)te.size(); counts[1] = (int64_t)tr.size();
+    if (tiles)
+        for (size_t i = 0; i < te.size(); ++i) {
+            tiles[4 * i] = te[i].slot; tiles[4 * i + 1] = te[i].ti; tiles[4 * i + 2] = te[i].tj; tiles[4 * i + 3] = te[i].rect;
+        }
+    if (rects)
+        for (size_t i = 0; i < tr.size(); ++i) {
+            const cb200::TileRect& r = tr[i];
+            rects[5 * i] = r.child; rects[5 * i + 1] = r.ja; rects[5 * i + 2] = r.jb; rects[5 * i + 3] = r.ia; rects[5 * i + 4] = r.ib;
+        }
+    return 0;
+}
+
 }  // extern "C"

@@ -7,8 +7,8 @@
 //   G4  small-front LDL' (shared memory)  k_factor_small (nf <= 64), k_factor_panel (64 < nf <= 152)
 //   G5  large-front blocked LDL'          k_piv_diag, k_piv_rows, k_ldl_update_tma (TMA-fed 128 x 128 DMMA GEMM),
 //                                         k_ldl_update_ldg (fallback), k_finish_large
-//   G6  extend-add                        fused in G4 ; k_assemble_large ; gather_update_tile (Schur epilogue) ;
-//                                         k_assemble_atomic
+//   G6  extend-add                        fused in G4 ; k_assemble_tiles ; add_tile_rects (also in the Schur
+//                                         epilogue) ; k_assemble_atomic
 //   G7  multifrontal triangular solves    k_fwd_{leaf,warp<16|32>,cta}, k_bwd_*, k_big_{asm,tri,gemv}_*, k_*_subtree,
 //                                         k_pack_perm, k_unpack_perm
 //   G8  symmetric SpMV residual + norm    k_residual, k_residual_long
@@ -17,6 +17,7 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 #include <cuda.h>          // CUtensorMap (type only; the encoder is fetched through cudaGetDriverEntryPoint)
+#include "symbolic.h"      // MANY_CHILDREN, TileEntry, TileRect
 
 namespace cb200 {
 
@@ -45,8 +46,6 @@ __device__ __forceinline__ void note_reg(const RegParams& rp, unsigned int* nreg
     const unsigned int slot = atomicAdd(nreg, count);
     if (rp.log && slot < 64u) rp.log[slot] = col;
 }
-constexpr int MANY_CHILDREN = 2048;   // fronts with more children are assembled by k_assemble_atomic
-
 
 // ------------------------------------------------------------------ inverted diagonal blocks
 // The triangular solves never substitute column by column: every SBxSB diagonal block of the
@@ -354,48 +353,14 @@ k_factor_panel(DevSym S, const int32_t* __restrict__ batch, int maxpanel, int ma
 
 // ------------------------------------------------------------------ G6 assembly for large fronts
 // Large fronts come in two kinds.  A gather front (the default: at most MANY_CHILDREN children, not a
-// replicated top front) has only its panel columns assembled here; its update block U is never zeroed
-// or pre-assembled: the Schur epilogue builds each tile of U from the children (gather_update_tile)
-// and writes U = sum - L21 D L21' once.  A pre-assembled front (more than MANY_CHILDREN children:
-// k_assemble_atomic; multi-GPU top fronts: summed by NCCL before the Schur GEMM) is zeroed
-// (k_zero_upd), fully assembled and then updated in place by the epilogue.
+// replicated top front) has only its panel columns assembled by k_assemble_tiles; its update block U
+// is never zeroed or pre-assembled: the Schur epilogue builds each tile of U from the children
+// (add_tile_rects) and writes U = sum - L21 D L21' once.  A pre-assembled front (more than
+// MANY_CHILDREN children: k_assemble_atomic; multi-GPU top fronts: summed by NCCL before the Schur
+// GEMM) is zeroed (k_zero_upd), fully assembled and then updated in place by the epilogue.
+// Both walk host-built per-tile rectangle lists (symbolic.h, build_tile_lists).
 __device__ __forceinline__ bool gathers_update(const DevSym& S, int s, int gather) {
     return gather && S.child_ptr[s + 1] - S.child_ptr[s] <= MANY_CHILDREN;
-}
-
-// grid (ceil(maxnf / 8), nbatch) (ceil(maxns / 8) for a gather batch), 256 threads: one warp per
-// destination column of the front; sources ordered by child (deterministic), no inter-warp
-// conflicts, no barriers.
-constexpr int ASM_CW = 8;
-__global__ void __launch_bounds__(256)
-k_assemble_large(DevSym S, const int32_t* __restrict__ batch, int gather, double* __restrict__ Lst,
-                 double* __restrict__ Ust) {
-    const int s = batch[blockIdx.y];
-    const int f = S.sn_first[s];
-    const int ns = S.sn_first[s + 1] - f;
-    const int nr = (int)(S.rows_ptr[s + 1] - S.rows_ptr[s]);
-    const int nf = ns + nr;
-    const int ld = S.ld[s];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const int d = blockIdx.x * ASM_CW + wid;
-    if (d >= (gather ? ns : nf)) return;
-    if (S.child_ptr[s + 1] - S.child_ptr[s] > MANY_CHILDREN) return;     // k_assemble_atomic
-    double* Lp = Lst + S.panel_off[s];
-    double* Us = Ust + S.upd_off[s];
-    double* dst = d < ns ? Lp + (int64_t)d * ld : Us + (int64_t)(d - ns) * nr - ns;
-    const int32_t* cp = S.asm_colptr + S.front_ptr[s];
-    const int64_t base = S.asm_base[s];
-    for (int e = cp[d]; e < cp[d + 1]; ++e) {
-        const int q = S.asm_src[base + e];
-        const int c = S.asm_child[base + e];
-        if (S.active && !S.active[c]) continue;
-        const int64_t rp0 = S.rows_ptr[c];
-        const int nrc = (int)(S.rows_ptr[c + 1] - rp0);
-        const int j = (int)(q - rp0);
-        const int32_t* relc = S.rel + rp0;
-        const double* src = Ust + S.upd_off[c] + (int64_t)j * nrc;
-        for (int i = j + lane; i < nrc; i += 32) dst[relc[i]] += src[i];
-    }
 }
 
 // Fronts with thousands of (tiny) children — e.g. the factor-row front of a portfolio KKT system
@@ -470,10 +435,10 @@ __device__ __forceinline__ void dmma16816(double (&c)[4], const double (&a)[8], 
 // with k in [k0, k1).  Tiles of size T are anchored at front-local index 0.
 //   mode 0 (panel step at pivot block J0): k = [J0, min(J0+PB, ns)), cols (k1, ns);  grid.x = nb * na,
 //          tile (tj0 + b, tj0 + b + a) for b = x / na, a = x % na
-//   mode 1 (Schur): k = [0, ns), cols [ns, nf);  grid.x = T (T + 1) / 2 triangular over tiles >= tj0
+//   mode 1 (Schur): k = [0, ns), cols [ns, nf);  grid.x = the batch's Schur tile list (build_tile_lists)
 struct UpdTile { int k0, k1, c_lo, c_hi, ti, tj; bool valid; };
 template <int T>
-__device__ __forceinline__ UpdTile decode_update_tile(int mode, int J0, int na, int ns, int nf) {
+__device__ __forceinline__ UpdTile decode_update_tile(int mode, int J0, int na, int ns, int nf, const TileEntry& te) {
     UpdTile u; u.valid = false;
     if (mode == 0) {
         if (J0 >= ns) return u;
@@ -481,17 +446,11 @@ __device__ __forceinline__ UpdTile decode_update_tile(int mode, int J0, int na, 
         if (u.c_lo >= u.c_hi) return u;
         const int tj0 = u.c_lo / T;
         u.tj = tj0 + (int)blockIdx.x / na; u.ti = u.tj + (int)blockIdx.x % na;
-    } else {
-        if (nf == ns) return u;
+        u.valid = (u.tj * T < u.c_hi) && (u.ti * T < nf);
+    } else {                                    // every listed tile is a valid one
         u.k0 = 0; u.k1 = ns; u.c_lo = ns; u.c_hi = nf;
-        const int tj0 = u.c_lo / T;
-        const int idx = blockIdx.x;
-        int a = (int)((sqrt(8.0 * idx + 1.0) - 1.0) * 0.5);
-        while ((a + 1) * (a + 2) / 2 <= idx) ++a;
-        while (a * (a + 1) / 2 > idx) --a;
-        u.ti = tj0 + a; u.tj = tj0 + idx - a * (a + 1) / 2;
+        u.ti = te.ti; u.tj = te.tj; u.valid = true;
     }
-    u.valid = (u.tj * T < u.c_hi) && (u.ti * T < nf);
     return u;
 }
 
@@ -500,53 +459,87 @@ __device__ __forceinline__ UpdTile decode_update_tile(int mode, int J0, int na, 
 template <int T>
 __device__ __forceinline__ int tile_idx(int r, int c) { return c * T + (r ^ (((c >> 1) & 3) << 3)); }
 
-// Schur epilogue of a gather front: builds the tile (rows r0.., columns c0..) of the sum of the
-// children's contributions to U in shared memory, in the order of k_assemble_large (every entry is
-// 0 + c1 + c2 + ... over the sources of its column in child order), so that U = tile - acc is
-// bitwise what assembling U first and updating it in place gives.  Warp w of the nthr / 32 walks the
-// front columns c0 + w, c0 + w + nthr / 32, ...  The child rows of a source that land in the row
-// window start at the lower bound of r0 in the child's ascending rel; the bound does not depend on
-// the column, so each warp keeps the last child's.  sync() synchronises the nthr threads; the first
-// one lets the tile alias buffers the threads were still reading.
+// Adds the rectangles rect[0..nrect) of a tile (rows r0.., columns c0..) into the T x T tile in
+// shared memory, one after the other: every entry becomes start + c1 + c2 + ... in child_list order,
+// the order of the destination-owner maps.  The entries of one rectangle are distinct, so its
+// threads need no ordering among themselves; a barrier separates consecutive rectangles.  Each
+// rectangle's rel windows are staged in relw (2 x 2T ints, double-buffered so that one barrier per
+// rectangle suffices): child rows [ia, ib) -> tile rows, child columns [ja, jb) -> tile columns.
+// Every rectangle is processed, so that buffer k & 1 is never restaged before the barrier that
+// ends its last use: the multi-GPU mask of inactive children is applied when the lists are built.
+// Warp w adds child columns ja + w, ja + w + nthr / 32, ...; their rows are contiguous and ascending
+// in the child's update block.  sync() synchronises the nthr threads; the last one publishes the tile.
 template <int T, class Sync>
-__device__ __forceinline__ void gather_update_tile(const DevSym& S, int s, int ns, int nf,
-                                                   const double* __restrict__ Ust, int r0, int c0,
-                                                   double* tile, int tid, int nthr, Sync sync) {
-    sync();
-    for (int e = tid; e < T * T; e += nthr) tile[e] = 0.0;
-    sync();
+__device__ __forceinline__ void add_tile_rects(const DevSym& S, const double* __restrict__ Ust,
+                                               const TileRect* __restrict__ rect, int nrect, int r0, int c0,
+                                               double* tile, int* relw, int tid, int nthr, Sync sync) {
     const int lane = tid & 31;
-    const int32_t* cp = S.asm_colptr + S.front_ptr[s];
-    const int64_t base = S.asm_base[s];
-    int cc = -1, clb = 0;                          // child whose lower bound of r0 is known, and the bound
-    for (int dl = tid >> 5; dl < T; dl += nthr >> 5) {
-        const int d = c0 + dl;
-        if (d < ns || d >= nf) continue;
-        for (int e = cp[d]; e < cp[d + 1]; ++e) {
-            const int c = S.asm_child[base + e];
-            if (S.active && !S.active[c]) continue;
-            const int64_t rp0 = S.rows_ptr[c];
-            const int nrc = (int)(S.rows_ptr[c + 1] - rp0);
-            const int j = (int)(S.asm_src[base + e] - rp0);
-            const int32_t* relc = S.rel + rp0;
-            int i0 = j;                            // child row j is front row d; rows below it map below d
-            if (r0 > d) {
-                if (c != cc) {
-                    int lo = j, hi = nrc;
-                    while (lo < hi) { const int m = (lo + hi) >> 1; if (relc[m] < r0) lo = m + 1; else hi = m; }
-                    cc = c; clb = lo;
-                }
-                i0 = max(j, clb);
-            }
-            const double* src = Ust + S.upd_off[c] + (int64_t)j * nrc;
-            for (int i = i0 + lane; i < nrc; i += 32) {
-                const int r = relc[i] - r0;
-                if (r >= T) break;
-                tile[tile_idx<T>(r, dl)] += src[i];
-            }
+    for (int k = 0; k < nrect; ++k) {
+        const int4 a = __ldg(reinterpret_cast<const int4*>(rect + k));          // child, ja, jb, ia
+        const int c = a.x, ja = a.y, jb = a.z, ia = a.w, ib = __ldg(&rect[k].ib);
+        const int64_t rp0 = S.rows_ptr[c];
+        const int nrc = (int)(S.rows_ptr[c + 1] - rp0);
+        const int32_t* relc = S.rel + rp0;
+        const double* src = Ust + S.upd_off[c];
+        int* rw = relw + (k & 1) * 2 * T;
+        for (int e = tid; e < ib - ia; e += nthr) rw[e] = relc[ia + e] - r0;
+        for (int e = tid; e < jb - ja; e += nthr) rw[T + e] = relc[ja + e] - c0;
+        sync();
+        for (int j = ja + (tid >> 5); j < jb; j += nthr >> 5) {
+            const int dl = rw[T + j - ja];
+            const double* sc = src + (int64_t)j * nrc;
+            const int i0 = max(ia, j) + lane;
+            double v[T / 32];
+#pragma unroll
+            for (int u = 0; u < T / 32; ++u) v[u] = i0 + 32 * u < ib ? sc[i0 + 32 * u] : 0.0;
+#pragma unroll
+            for (int u = 0; u < T / 32; ++u)
+                if (i0 + 32 * u < ib) tile[tile_idx<T>(rw[i0 + 32 * u - ia], dl)] += v[u];
         }
     }
     sync();
+}
+
+// One 64 x 64 tile of the panel columns of a gather front, or of any column of a pre-assembled front,
+// per CTA (the batch's assembly tile list): the tile is read as k_scatter / k_zero_upd left it, the
+// children's rectangles are added, and each entry is stored once.  256 threads.
+constexpr int ASM_T = 64;
+__global__ void __launch_bounds__(256)
+k_assemble_tiles(DevSym S, const int32_t* __restrict__ batch, const TileEntry* __restrict__ tiles,
+                 const TileRect* __restrict__ rects, int gather, double* __restrict__ Lst, double* __restrict__ Ust) {
+    __shared__ double tile[ASM_T * ASM_T];
+    __shared__ int relw[4 * ASM_T];
+    const TileEntry te = tiles[blockIdx.x];
+    const int rend = tiles[blockIdx.x + 1].rect;
+    const int s = batch[te.slot];
+    const int ns = S.sn_first[s + 1] - S.sn_first[s];
+    const int nr = (int)(S.rows_ptr[s + 1] - S.rows_ptr[s]);
+    const int nf = ns + nr;
+    const int ld = S.ld[s];
+    const int chi = gathers_update(S, s, gather) ? ns : nf;        // a gather front's U is built by the Schur epilogue
+    double* Lp = Lst + S.panel_off[s];
+    double* Us = Ust + S.upd_off[s];
+    const int r0 = te.ti * ASM_T, c0 = te.tj * ASM_T;
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    auto column = [&](int d) { return d < ns ? Lp + (int64_t)d * ld : Us + (int64_t)(d - ns) * nr - ns; };
+    for (int dl = wid; dl < ASM_T && c0 + dl < chi; dl += 8) {
+        const double* col = column(c0 + dl);
+#pragma unroll
+        for (int u = 0; u < ASM_T / 32; ++u) {
+            const int r = r0 + lane + 32 * u;
+            if (r >= c0 + dl && r < nf) tile[tile_idx<ASM_T>(lane + 32 * u, dl)] = col[r];
+        }
+    }
+    add_tile_rects<ASM_T>(S, Ust, rects + te.rect, rend - te.rect, r0, c0, tile, relw, tid, 256,
+                          [] { __syncthreads(); });
+    for (int dl = wid; dl < ASM_T && c0 + dl < chi; dl += 8) {
+        double* col = column(c0 + dl);
+#pragma unroll
+        for (int u = 0; u < ASM_T / 32; ++u) {
+            const int r = r0 + lane + 32 * u;
+            if (r >= c0 + dl && r < nf) col[r] = tile[tile_idx<ASM_T>(lane + 32 * u, dl)];
+        }
+    }
 }
 
 // acc (4 x 4 per thread, rows tx*4+a, cols ty*4+c) = sum_{k in [k0,k1)} L[rowA0+i, k] D[k] L[rowB0+j, k]
@@ -634,24 +627,30 @@ __device__ __forceinline__ void ldl_gemm_tile(const double* __restrict__ Lp, int
 }
 
 __global__ void __launch_bounds__(256)
-k_ldl_update_ldg(DevSym S, const int32_t* __restrict__ batch, int mode, int J0, int na, int gather,
+k_ldl_update_ldg(DevSym S, const int32_t* __restrict__ batch, const TileEntry* __restrict__ tiles,
+                 const TileRect* __restrict__ rects, int mode, int J0, int na, int gather,
                  double* __restrict__ Lst, double* __restrict__ Ust, const double* __restrict__ D) {
     __shared__ double gsm[GSM];
+    __shared__ int relw[4 * GBM];
     static_assert(GBM * GBM <= GSM, "the gathered tile aliases the operand buffers");
-    const int s = batch[blockIdx.y];
+    const TileEntry te = mode == 1 ? tiles[blockIdx.x] : TileEntry{(int32_t)blockIdx.y, 0, 0, 0};
+    const int s = batch[te.slot];
     const int f = S.sn_first[s];
     const int ns = S.sn_first[s + 1] - f;
     const int nr = (int)(S.rows_ptr[s + 1] - S.rows_ptr[s]);
     const int nf = ns + nr;
     const int ld = S.ld[s];
-    const UpdTile u = decode_update_tile<GBM>(mode, J0, na, ns, nf);
+    const UpdTile u = decode_update_tile<GBM>(mode, J0, na, ns, nf, te);
     if (!u.valid) return;
     double* Lp = Lst + S.panel_off[s];
     double acc[4][4];
     ldl_gemm_tile(Lp, ld, nf, D + f, u.ti * GBM, u.tj * GBM, u.k0, u.k1, acc, gsm);
     const bool gat = mode == 1 && gathers_update(S, s, gather);
-    if (gat) gather_update_tile<GBM>(S, s, ns, nf, Ust, u.ti * GBM, u.tj * GBM, gsm, threadIdx.x, 256,
-                                     [] { __syncthreads(); });
+    if (gat) {                                  // the tile aliases the operand buffers (free after ldl_gemm_tile)
+        for (int e = threadIdx.x; e < GBM * GBM; e += 256) gsm[e] = 0.0;
+        add_tile_rects<GBM>(S, Ust, rects + te.rect, tiles[blockIdx.x + 1].rect - te.rect, u.ti * GBM, u.tj * GBM,
+                            gsm, relw, threadIdx.x, 256, [] { __syncthreads(); });
+    }
     double* Us = Ust + S.upd_off[s];
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
     double cv[4][4];
@@ -687,7 +686,10 @@ constexpr int TSTAGES = 4;
 // tile T x T: consumer warps (T/64 x T/32 for T = 128: warp tile 64 x 32; 2 x 2 for T = 64: warp tile 32 x 32)
 // plus one producer warp
 constexpr int tma_threads(int T) { return (T == 128 ? 8 : 4) * 32 + 32; }
-constexpr size_t tma_gemm_smem(int T) { return (size_t)TSTAGES * 2 * T * TK * sizeof(double) + 2 * TSTAGES * sizeof(uint64_t); }
+// stage ring (the gathered tile aliases it), full / empty barriers, rel windows of add_tile_rects
+constexpr size_t tma_gemm_smem(int T) {
+    return (size_t)TSTAGES * 2 * T * TK * sizeof(double) + 2 * TSTAGES * sizeof(uint64_t) + 4 * T * sizeof(int);
+}
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -721,18 +723,20 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
 // (sk, srg) - same kernel, 4-way bank conflicts on the fragment loads.
 template <int T>
 __global__ void __launch_bounds__(tma_threads(T), T == 128 ? 1 : 3)
-k_ldl_update_tma(DevSym S, const int32_t* __restrict__ batch, const CUtensorMap* __restrict__ maps,
+k_ldl_update_tma(DevSym S, const int32_t* __restrict__ batch, const TileEntry* __restrict__ tiles,
+                 const TileRect* __restrict__ rects, const CUtensorMap* __restrict__ maps,
                  const int32_t* __restrict__ map_of, int mode, int J0, int na, int gather, int kmajor,
                  double* __restrict__ Lst, double* __restrict__ Ust, const double* __restrict__ D) {
     extern __shared__ __align__(128) unsigned char tma_smem[];
     static_assert(T * T <= 2 * TSTAGES * T * TK, "the gathered tile aliases the stage ring");
-    const int s = batch[blockIdx.y];
+    const TileEntry te = mode == 1 ? tiles[blockIdx.x] : TileEntry{(int32_t)blockIdx.y, 0, 0, 0};
+    const int s = batch[te.slot];
     const int f = S.sn_first[s];
     const int ns = S.sn_first[s + 1] - f;
     const int nr = (int)(S.rows_ptr[s + 1] - S.rows_ptr[s]);
     const int nf = ns + nr;
     const int ld = S.ld[s];
-    const UpdTile u = decode_update_tile<T>(mode, J0, na, ns, nf);
+    const UpdTile u = decode_update_tile<T>(mode, J0, na, ns, nf, te);
     if (!u.valid) return;
     double* sA = reinterpret_cast<double*>(tma_smem);
     constexpr int TTILE = T * TK;                      // doubles per operand per stage
@@ -827,8 +831,14 @@ k_ldl_update_tma(DevSym S, const int32_t* __restrict__ batch, const CUtensorMap*
     // A gather front's U tile is built in the stage ring instead: every stage has been waited on, so
     // no TMA write is in flight, and the producer warp has returned (named barrier 1, consumers only).
     const bool gat = mode == 1 && gathers_update(S, s, gather);
-    if (gat) gather_update_tile<T>(S, s, ns, nf, Ust, u.ti * T, u.tj * T, sA, tid, NCW * 32,
-                                   [] { asm volatile("bar.sync 1, %0;\n" :: "n"(NCW * 32) : "memory"); });
+    if (gat) {
+        auto sync = [] { asm volatile("bar.sync 1, %0;\n" :: "n"(NCW * 32) : "memory"); };
+        sync();                                        // every consumer is done reading the ring
+        for (int e = tid; e < T * T; e += NCW * 32) sA[e] = 0.0;
+        const int rb = tiles[blockIdx.x].rect;
+        add_tile_rects<T>(S, Ust, rects + rb, tiles[blockIdx.x + 1].rect - rb, u.ti * T, u.tj * T, sA,
+                          reinterpret_cast<int*>(empty + TSTAGES), tid, NCW * 32, sync);
+    }
     double* Lp = Lst + S.panel_off[s];
     double* Us = Ust + S.upd_off[s];
 #pragma unroll

@@ -595,4 +595,52 @@ void partition_subtrees(const Symbolic& S, int32_t nranks, std::vector<int32_t>&
     if (rank_load) *rank_load = load;
 }
 
+void build_tile_lists(const Symbolic& S, const int32_t* fronts, int32_t n, int32_t T, bool schur,
+                      bool gather, const int8_t* active, std::vector<TileEntry>& tiles,
+                      std::vector<TileRect>& rects) {
+    std::vector<int32_t> bnd;                        // per child: first child row at or below each tile boundary
+    for (int32_t k = 0; k < n; ++k) {
+        const int32_t s = fronts[k];
+        const int32_t ns = S.ns(s), nf = ns + S.nr(s);
+        const int32_t c0 = S.child_ptr[s], nch = S.child_ptr[s + 1] - c0;
+        const bool gathers = gather && nch <= MANY_CHILDREN;
+        if (schur ? nf == ns : (nch > MANY_CHILDREN || nch == 0)) continue;
+        const int32_t nt = (nf - 1) / T + 1;          // tiles per side
+        const int32_t nb = nt + 2;                    // boundaries 0..nt, then lower_bound(ns)
+        const bool with_rects = !schur || gathers;
+        if (with_rects) {
+            bnd.assign((size_t)nch * nb, 0);
+            for (int32_t q = 0; q < nch; ++q) {
+                const int32_t c = S.child_list[c0 + q];
+                if (active && !active[c]) continue;
+                const int32_t* relc = S.rel.data() + S.rows_ptr[c];
+                const int32_t nrc = S.nr(c);
+                int32_t* b = bnd.data() + (size_t)q * nb;
+                for (int32_t t = 0, i = 0; t <= nt; ++t) {
+                    while (i < nrc && relc[i] < t * T) ++i;
+                    b[t] = i;
+                }
+                b[nt + 1] = (int32_t)(std::lower_bound(relc, relc + nrc, ns) - relc);
+            }
+        }
+        const int32_t chi = schur ? nf : (gathers ? ns : nf);      // columns [clo, chi) are assembled here
+        const int32_t clo = schur ? ns : 0;
+        for (int32_t tj = clo / T; tj * T < chi; ++tj)
+            for (int32_t ti = tj; ti < nt; ++ti) {
+                const size_t r0 = rects.size();
+                if (with_rects)
+                    for (int32_t q = 0; q < nch; ++q) {
+                        if (active && !active[S.child_list[c0 + q]]) continue;
+                        const int32_t* b = bnd.data() + (size_t)q * nb;
+                        const int32_t nrc = S.nr(S.child_list[c0 + q]);
+                        const int32_t ja = std::max(b[tj], schur ? b[nt + 1] : 0);
+                        const int32_t ia = b[ti], ib = b[ti + 1];
+                        const int32_t jb = std::min({b[tj + 1], ib, chi == ns ? b[nt + 1] : nrc});
+                        if (ja < jb && ia < ib) rects.push_back({S.child_list[c0 + q], ja, jb, ia, ib, {0, 0, 0}});
+                    }
+                if (schur || rects.size() > r0) tiles.push_back({k, ti, tj, (int32_t)r0});
+            }
+    }
+}
+
 }  // namespace cb200

@@ -44,6 +44,7 @@ inline bool front_is_large(const SymbolicOptions& o, int nf, int ns) {
     return nf > o.small_max_nf && !front_to_panel(o, nf, ns);
 }
 constexpr int32_t LD_ALIGN = 8;
+constexpr int MANY_CHILDREN = 2048;   // large fronts with more children are assembled by k_assemble_atomic
 
 struct Symbolic {
     int64_t N = 0, nnzK = 0;
@@ -87,6 +88,27 @@ struct Symbolic {
     inline int32_t ns(int32_t s) const { return sn_first[s + 1] - sn_first[s]; }
     inline int32_t nr(int32_t s) const { return (int32_t)(rows_ptr[s + 1] - rows_ptr[s]); }
 };
+
+// Per-tile source lists of the large-front extend-add.  A child's rel is ascending, so what it adds
+// to a T x T tile (rows r0.., columns c0..) of its parent is a rectangle of its update block: child
+// columns [ja, jb), and rows [max(ia, j), ib) of column j.  A tile entry names the front (its slot in
+// the batch), the tile and its first rectangle; its rectangles end where the next entry's begin (the
+// lists end with a sentinel entry).  Rectangles of a tile are in child_list order, so adding them one
+// after the other sums every entry in the order of the destination-owner maps.
+struct TileEntry { int32_t slot, ti, tj, rect; };
+struct TileRect { int32_t child, ja, jb, ia, ib, pad[3]; };
+// Appends the tiles of the batch fronts[0..n) to `tiles` / `rects` (slot = position in fronts).
+//   schur: every tile (ti >= tj) of columns [ns, nf) of the fronts with nr > 0 - the Schur GEMM's tiles.
+//          Only fronts that gather their update block (gather and at most MANY_CHILDREN children)
+//          get rectangles, restricted to columns >= ns; the others are updated in place.
+//   else:  the tiles of columns [0, ns) (gather) or [0, nf) (pre-assembled fronts) that some child
+//          reaches; fronts with more than MANY_CHILDREN children are left to k_assemble_atomic.
+// active (multi-GPU, nullptr = all): per-supernode mask of the children whose contributions this
+// rank assembles; the other children get no rectangles.
+// The caller appends the sentinel {0, 0, 0, rects.size()} after the last batch.
+void build_tile_lists(const Symbolic& S, const int32_t* fronts, int32_t n, int32_t T, bool schur,
+                      bool gather, const int8_t* active, std::vector<TileEntry>& tiles,
+                      std::vector<TileRect>& rects);
 
 // Multi-GPU partition of the assembly tree (SURVEY.md section 8e): an upward-closed "top" set of
 // supernodes (root separator fronts) is replicated on every rank; the subtrees hanging below it

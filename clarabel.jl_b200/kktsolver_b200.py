@@ -113,11 +113,11 @@ class B200DirectLDLSolver:
         return {self._L.cb200_fine_timer_name(i).decode(): float(out[i]) for i in range(n)}
 
     def stats(self):
-        out = np.zeros(17)
-        self._L.cb200_get_stats(self._h, _p(out), 17)
+        out = np.zeros(21)
+        self._L.cb200_get_stats(self._h, _p(out), 21)
         keys = ["flops", "schur_flops", "panel_flops", "nnzL", "nlevels", "nsuper", "nlarge",
                 "big_solve_bytes", "upd_bytes", "panel_bytes", "ordering_used", "rank_flops", "use_tma", "tma_kmajor",
-                "factor_graphs", "solve_graph", "subtrees"]
+                "factor_graphs", "solve_graph", "subtrees", "schur_tiles", "schur_rects", "asm_tiles", "asm_rects"]
         return dict(zip(keys, out.tolist()))
 
     def reset_timers(self):

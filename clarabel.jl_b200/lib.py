@@ -14,7 +14,7 @@ _LIB = None
 # every symbol include/clarabel_b200.h declares
 EXPORTED = [
     "cb200_default_settings", "cb200_symbolic_create", "cb200_symbolic_destroy",
-    "cb200_symbolic_stat", "cb200_symbolic_flops", "cb200_symbolic_get",
+    "cb200_symbolic_stat", "cb200_symbolic_flops", "cb200_symbolic_get", "cb200_symbolic_tile_lists",
     "cb200_order_amd", "cb200_order_nd",
     "cb200_create", "cb200_destroy", "cb200_update_values", "cb200_scale_values",
     "cb200_refactor", "cb200_solve", "cb200_info",
@@ -59,6 +59,8 @@ def lib():
         L.cb200_symbolic_stat.argtypes = [P, I32]; L.cb200_symbolic_stat.restype = I64
         L.cb200_symbolic_flops.argtypes = [P]; L.cb200_symbolic_flops.restype = D
         L.cb200_symbolic_get.argtypes = [P, I32, P, I64]; L.cb200_symbolic_get.restype = I32
+        L.cb200_symbolic_tile_lists.argtypes = [P, P, I32, I32, I32, I32, P, P, P, P]
+        L.cb200_symbolic_tile_lists.restype = I32
         L.cb200_order_amd.argtypes = [I64, P, P, D, P]; L.cb200_order_amd.restype = I32
         L.cb200_order_nd.argtypes = [I64, P, P, D, I64, P]; L.cb200_order_nd.restype = I32
         L.cb200_create.argtypes = [I64, P, P, P, P, P, P]; L.cb200_create.restype = I32
@@ -178,9 +180,7 @@ class Symbolic:
         out = {}
         lens["panel_ld"] = s["nsuper"]
         for i, nm in enumerate(_SYM_ARRAYS):
-            if nm == "child_list":
-                continue
-            a = np.empty(lens[nm], dtype=np.int64)
+            a = np.empty(lens[nm] if nm != "child_list" else out["child_ptr"][-1], dtype=np.int64)
             check(L.cb200_symbolic_get(self._h, i, _p(a), len(a)), "cb200_symbolic_get")
             out[nm] = a
         ch = [[] for _ in range(s["nsuper"])]
@@ -197,6 +197,23 @@ class Symbolic:
         check(lib().cb200_symbolic_partition(self._h, int(nranks), _p(owner), _p(top), _p(load)),
               "cb200_symbolic_partition")
         return owner, top.astype(bool), load
+
+    def tile_lists(self, fronts, T, schur, gather=True, active=None):
+        """Per-tile source lists of the large-front extend-add for one batch of fronts:
+        tiles [n, 4] (slot, ti, tj, first rectangle; a final sentinel row holds the end) and
+        rects [m, 5] (child, ja, jb, ia, ib).  active: optional per-supernode mask (multi-GPU) of
+        the children whose contributions are assembled."""
+        L = lib()
+        fr = np.ascontiguousarray(fronts, dtype=np.int64)
+        act = None if active is None else np.ascontiguousarray(active, dtype=np.int64)
+        cnt = np.zeros(2, dtype=np.int64)
+        args = (self._h, _p(fr), len(fr), int(T), int(bool(schur)), int(bool(gather)), _p(act), _p(cnt))
+        check(L.cb200_symbolic_tile_lists(*args, None, None), "cb200_symbolic_tile_lists")
+        tiles = np.zeros((cnt[0] + 1, 4), dtype=np.int64)
+        rects = np.zeros((cnt[1], 5), dtype=np.int64)
+        check(L.cb200_symbolic_tile_lists(*args, _p(tiles), _p(rects)), "cb200_symbolic_tile_lists")
+        tiles[-1, 3] = cnt[1]
+        return tiles, rects
 
     def __del__(self):
         try:

@@ -70,6 +70,16 @@ double  cb200_symbolic_flops(const cb200_symbolic* s);
  *        8 a_map[nnzK], 9 sn_level[nsuper], 10 child_ptr[nsuper+1], 11 child_list[nsuper-#roots]
  * All arrays are returned widened to int64 into caller storage of the stated length. */
 int32_t cb200_symbolic_get(const cb200_symbolic* s, int32_t which, int64_t* out, int64_t len);
+/* Per-tile source lists of the large-front extend-add (symbolic.h, build_tile_lists) for the batch
+ * fronts[0..nfronts) and tile size T (64 or 128): schur = 1 the Schur GEMM's tiles, 0 the assembly
+ * tiles; gather = 0 for pre-assembled (replicated top) fronts; active (NULL = all, else [nsuper], nonzero
+ * = assembled here): multi-GPU mask of the children whose contributions a rank adds, the others get no
+ * rectangles.  counts[0] = tiles, counts[1] =
+ * rectangles.  If non-NULL, tiles receives (slot, ti, tj, first rectangle) per tile and rects
+ * (child, ja, jb, ia, ib) per rectangle; call once with NULL to size them. */
+int32_t cb200_symbolic_tile_lists(const cb200_symbolic* s, const int64_t* fronts, int32_t nfronts, int32_t T,
+                                  int32_t schur, int32_t gather, const int64_t* active, int64_t* counts,
+                                  int64_t* tiles, int64_t* rects);
 
 /* Multi-GPU partition of the assembly tree (host-only): owner[s] in [0,nranks) or -1 for the
  * replicated top set, is_top[s] in {0,1}, rank_load[nranks] = factor-flop weight per rank. */
@@ -166,7 +176,8 @@ const char* cb200_fine_timer_name(int32_t i);
  * fronts, 7 panel bytes of the multi-CTA solve class, 8 update-storage bytes, 9 panel-storage bytes,
  * 10 ordering used, 11 flops of this rank's fronts, 12 TMA tensor maps in use, 13 their k-major order,
  * 14 factorisation graphs instantiated (0-2), 15 solve-sweep graph instantiated, 16 bottom subtrees
- * solved by k_fwd_subtree / k_bwd_subtree */
+ * solved by k_fwd_subtree / k_bwd_subtree, 17 Schur tiles and 18 their child rectangles, 19 assembly
+ * tiles and 20 their child rectangles (all large batches, cb200_symbolic_tile_lists) */
 int32_t cb200_get_stats(const cb200_handle* h, double* out, int32_t len);
 /* ---------------------------------------------------------------- multi-GPU (one process per GPU)
  * Every rank creates the same handle on its own device (replicated symbolic analysis), then
