@@ -5,6 +5,7 @@
 #include "symbolic.h"
 #include "api_common.h"
 #include "kernels.cuh"
+#include "kernels_multi.cuh"
 
 #include <dlfcn.h>
 #include <nccl.h>
@@ -284,6 +285,17 @@ struct cb200_handle {
     DevBuf<int64_t> d_stage_idx; DevBuf<double> d_stage_val;
     size_t stage_idx_cap = 0, stage_val_cap = 0;
     Timers tm;
+    // multi-right-hand-side state (cb200_solve_multi / cb200_solve_ir_multi): grow-only, allocated by the first
+    // multi call, so a caller that never uses those entry points pays no memory
+    int multi_w = 0;                                // widest sweep (1, 2 or 4; shared memory can cap it), 0: not allocated
+    DevBuf<double> d_my, d_muvec, d_mpartial;       // interleaved sweep vectors (R > 1; R = 1 uses d_y, d_uvec, d_partial)
+    DevBuf<double> d_mb, d_mx, d_mdx, d_me;         // interleaved refinement vectors, N x multi_w
+    DevBuf<double> d_mstage, d_mrx, d_mrz;          // column-major staging of one chunk of the caller's columns
+    DevBuf<double> d_msol; int64_t msol_cols = 0;   // solutions of the last cb200_solve_ir_multi (download selector 8)
+    DevBuf<unsigned long long> d_mscal;             // [0, 4): ||b_r||_inf, [4, 8): ||e_r||_inf (bits)
+    GraphExec g_msolve[2];                          // sweep graphs of width 2 and 4 (width 1 is g_solve)
+    int64_t partial_len = 1;                        // doubles of d_partial (one column)
+    double n_multi_sweeps = 0, n_percol = 0;        // cb200_get_stats 21 / 22
 };
 
 namespace {
@@ -322,7 +334,13 @@ int launch_small(cb200_handle* h, const Batch& b, int cls, RegParams rp, cudaStr
     return 0;
 }
 
-void launch_fwd_level(cb200_handle* h, const LevelPlan& P, int lv) {
+// The work vectors of one sweep: R = 1 the single-column buffers, R > 1 the interleaved multi-RHS ones
+struct SweepBufs { double* y; double* uvec; double* partial; };
+// the single-column kernel for R = 1, its R-wide form (kernels_multi.cuh) otherwise; both take the same arguments
+#define PICK(R, single, multi) ([] { if constexpr (R == 1) return single; else return multi; }())
+
+template <int R>
+void launch_fwd_level(cb200_handle* h, const LevelPlan& P, int lv, const SweepBufs& V) {
     DevSym ds = devsym(h);
     // classes of a level are independent: leaf + tiny on side[0], warp on side[1], CTA on side[2], big on the
     // main stream (fork/join only when a second class has work)
@@ -335,32 +353,32 @@ void launch_fwd_level(cb200_handle* h, const LevelPlan& P, int lv) {
     const Batch& b0 = P.solve[0];
     if (b0.cnt) {
         { FineScope fs(h, Timers::F_FWD_LEAF);
-        k_fwd_leaf<<<nblk(b0.cnt, 128), 128, 0, s_leaf>>>(ds, h->d_batches.p + b0.off, b0.cnt, h->d_L.p,
-                                                             h->d_y.p, h->d_uvec.p);
+        PICK(R, k_fwd_leaf, k_fwd_leaf_multi<R>)<<<nblk(b0.cnt, 128), 128, 0, s_leaf>>>(ds, h->d_batches.p + b0.off, b0.cnt, h->d_L.p,
+                                                             V.y, V.uvec);
         LAUNCH(h);
         }
     }
     const Batch& b1 = P.solve[1];
     if (b1.cnt) {
         FineScope fs(h, Timers::F_FWD_WARP);
-        k_fwd_warp<32, false><<<nblk(b1.cnt, WPB), WPB * 32, (size_t)WPB * b1.maxnf * sizeof(double), s_warp>>>(
-            ds, h->d_sdesc.p + b1.off, b1.cnt, b1.maxnf, h->d_L.p, h->d_y.p, h->d_uvec.p);
+        PICK(R, (k_fwd_warp<32, false>), (k_fwd_warp_multi<32, R>))<<<nblk(b1.cnt, WPB), WPB * 32, fwd_warp_smem(b1.maxnf, R), s_warp>>>(
+            ds, h->d_sdesc.p + b1.off, b1.cnt, b1.maxnf, h->d_L.p, V.y, V.uvec);
         LAUNCH(h);
     }
     const Batch& b5 = P.solve[5];
     if (b5.cnt) {
         FineScope fs(h, Timers::F_FWD_WARP);
-        if (h->merged_rows) k_fwd_warp<16, true><<<nblk(b5.cnt, WPB), WPB * 32, (size_t)WPB * b5.maxnf * sizeof(double), s_warp>>>(
-            ds, h->d_sdesc.p + b5.off, b5.cnt, b5.maxnf, h->d_L.p, h->d_y.p, h->d_uvec.p);
-        else k_fwd_warp<16, false><<<nblk(b5.cnt, WPB), WPB * 32, (size_t)WPB * b5.maxnf * sizeof(double), s_warp>>>(
-            ds, h->d_sdesc.p + b5.off, b5.cnt, b5.maxnf, h->d_L.p, h->d_y.p, h->d_uvec.p);
+        auto k = R > 1 ? PICK(R, (k_fwd_warp<16, true>), (k_fwd_warp_multi<16, R>))
+                       : h->merged_rows ? k_fwd_warp<16, true> : k_fwd_warp<16, false>;
+        k<<<nblk(b5.cnt, WPB), WPB * 32, fwd_warp_smem(b5.maxnf, R), s_warp>>>(
+            ds, h->d_sdesc.p + b5.off, b5.cnt, b5.maxnf, h->d_L.p, V.y, V.uvec);
         LAUNCH(h);
     }
     const Batch& b2 = P.solve[2];
     if (b2.cnt) {
         { FineScope fs(h, Timers::F_FWD_CTA);
-        k_fwd_cta<<<b2.cnt, 256, (size_t)b2.maxnf * sizeof(double), s_cta>>>(
-            ds, h->d_sdesc.p + b2.off, h->d_L.p, h->d_y.p, h->d_uvec.p);
+        PICK(R, k_fwd_cta, k_fwd_cta_multi<R>)<<<b2.cnt, 256, (size_t)b2.maxnf * R * sizeof(double), s_cta>>>(
+            ds, h->d_sdesc.p + b2.off, h->d_L.p, V.y, V.uvec);
         LAUNCH(h);
         }
     }
@@ -370,11 +388,11 @@ void launch_fwd_level(cb200_handle* h, const LevelPlan& P, int lv) {
         const int32_t* bl = h->d_batches.p + b3.off;
         { FineScope fs(h, Timers::F_FWD_BIG_ASM);
         if (b3.src_per_row >= 512)
-            k_big_asm_fwd<256><<<dim3(b3.maxnf, b3.cnt), 256, 0, h->stream>>>(ds, bl, h->d_y.p, h->d_uvec.p);
+            PICK(R, k_big_asm_fwd<256>, (k_big_asm_fwd_multi<256, R>))<<<dim3(b3.maxnf, b3.cnt), 256, 0, h->stream>>>(ds, bl, V.y, V.uvec);
         else if (b3.many_children)
-            k_big_asm_fwd<32><<<dim3(nblk((int64_t)b3.maxnf * 32, 256), b3.cnt), 256, 0, h->stream>>>(ds, bl, h->d_y.p, h->d_uvec.p);
+            PICK(R, k_big_asm_fwd<32>, (k_big_asm_fwd_multi<32, R>))<<<dim3(nblk((int64_t)b3.maxnf * 32, 256), b3.cnt), 256, 0, h->stream>>>(ds, bl, V.y, V.uvec);
         else
-            k_big_asm_fwd<1><<<dim3(nblk(b3.maxnf, 256), b3.cnt), 256, 0, h->stream>>>(ds, bl, h->d_y.p, h->d_uvec.p);
+            PICK(R, k_big_asm_fwd<1>, (k_big_asm_fwd_multi<1, R>))<<<dim3(nblk(b3.maxnf, 256), b3.cnt), 256, 0, h->stream>>>(ds, bl, V.y, V.uvec);
         LAUNCH(h);
         }
         if (pass == 1 && h->dist) {
@@ -383,11 +401,11 @@ void launch_fwd_level(cb200_handle* h, const LevelPlan& P, int lv) {
             const Symbolic& S = h->S;
             g_nccl.GroupStart();
             for (int32_t sn : h->h_top_by_level[lv]) {
-                double* yt = h->d_y.p + S.sn_first[sn];
-                g_nccl.AllReduce(yt, yt, (size_t)S.ns(sn), ncclDouble, ncclSum, h->comm, h->stream);
+                double* yt = V.y + (int64_t)S.sn_first[sn] * R;
+                g_nccl.AllReduce(yt, yt, (size_t)S.ns(sn) * R, ncclDouble, ncclSum, h->comm, h->stream);
                 if (S.nr(sn) > 0) {
-                    double* ut = h->d_uvec.p + S.rows_ptr[sn];
-                    g_nccl.AllReduce(ut, ut, (size_t)S.nr(sn), ncclDouble, ncclSum, h->comm, h->stream);
+                    double* ut = V.uvec + S.rows_ptr[sn] * R;
+                    g_nccl.AllReduce(ut, ut, (size_t)S.nr(sn) * R, ncclDouble, ncclSum, h->comm, h->stream);
                 }
             }
             g_nccl.GroupEnd();
@@ -395,19 +413,20 @@ void launch_fwd_level(cb200_handle* h, const LevelPlan& P, int lv) {
         {
             FineScope fs(h, Timers::F_FWD_BIG_TRI);
             unsigned* sy = h->d_bigsync.p + b3.sync_off;
-            k_big_tri_fwd<<<b3.nwork, 256, 0, h->stream>>>(ds, h->d_bigwork.p + b3.work_off, sy, sy + 2, h->d_bigsync.p,
-                                                            h->d_L.p, h->d_y.p);
+            PICK(R, k_big_tri_fwd, k_big_tri_fwd_multi<R>)<<<b3.nwork, 256, 0, h->stream>>>(ds, h->d_bigwork.p + b3.work_off, sy, sy + 2, h->d_bigsync.p,
+                                                            h->d_L.p, V.y);
             LAUNCH(h);
         }
         if (b3.ntile) {
             FineScope fs(h, Timers::F_FWD_BIG_GEMV);
-            k_big_gemv_fwd<<<b3.ntile, 256, 0, h->stream>>>(ds, h->d_bigwork.p + b3.tile_off, h->d_L.p, h->d_y.p, h->d_uvec.p);
+            PICK(R, k_big_gemv_fwd, k_big_gemv_fwd_multi<R>)<<<b3.ntile, 256, 0, h->stream>>>(ds, h->d_bigwork.p + b3.tile_off, h->d_L.p, V.y, V.uvec);
             LAUNCH(h);
         }
     }
     if (ms) h->join(3);
 }
-void launch_bwd_level(cb200_handle* h, const LevelPlan& P) {
+template <int R>
+void launch_bwd_level(cb200_handle* h, const LevelPlan& P, const SweepBufs& V) {
     DevSym ds = devsym(h);
     const bool big_work = P.solve[3].cnt || P.tops.cnt;
     const int nclass = (P.solve[0].cnt || P.solve[4].cnt) + (P.solve[1].cnt != 0 || P.solve[5].cnt != 0) + (P.solve[2].cnt != 0) + big_work;
@@ -420,46 +439,46 @@ void launch_bwd_level(cb200_handle* h, const LevelPlan& P) {
         if (!b3.cnt) continue;
         if (b3.ntile) {
             FineScope fs(h, Timers::F_BWD_BIG_GEMV);
-            k_big_gemvT_bwd<<<b3.ntile, 256, 0, h->stream>>>(ds, h->d_bigwork.p + b3.tile_off, h->d_L.p, h->d_y.p,
-                                                              h->d_partial.p);
+            PICK(R, k_big_gemvT_bwd, k_big_gemvT_bwd_multi<R>)<<<b3.ntile, 256, 0, h->stream>>>(ds, h->d_bigwork.p + b3.tile_off, h->d_L.p, V.y,
+                                                              V.partial);
             LAUNCH(h);
         }
         FineScope fs(h, Timers::F_BWD_BIG_TRI);
         unsigned* sy = h->d_bigsync.p + b3.sync_off;
-        k_big_tri_bwd<<<b3.nwork, 256, 0, h->stream>>>(ds, h->d_bigwork.p + b3.work_off + b3.nwork, sy + 1,
+        PICK(R, k_big_tri_bwd, k_big_tri_bwd_multi<R>)<<<b3.nwork, 256, 0, h->stream>>>(ds, h->d_bigwork.p + b3.work_off + b3.nwork, sy + 1,
                                                         sy + 2 + b3.nwork, h->d_bigsync.p, h->d_L.p, h->d_Dinv.p,
-                                                        h->d_partial.p, h->d_y.p);
+                                                        V.partial, V.y);
         LAUNCH(h);
     }
     const Batch& b2 = P.solve[2];
     if (b2.cnt) {
         { FineScope fs(h, Timers::F_BWD_CTA);
-        k_bwd_cta<<<b2.cnt, 256, (size_t)b2.maxnf * sizeof(double), s_cta>>>(
-            ds, h->d_batches.p + b2.off, h->d_L.p, h->d_Dinv.p, h->d_y.p);
+        PICK(R, k_bwd_cta, k_bwd_cta_multi<R>)<<<b2.cnt, 256, R == 1 ? (size_t)b2.maxnf * sizeof(double) : bwd_cta_smem(b2.maxnf, R), s_cta>>>(
+            ds, h->d_batches.p + b2.off, h->d_L.p, h->d_Dinv.p, V.y);
         LAUNCH(h);
         }
     }
     const Batch& b1 = P.solve[1];
     if (b1.cnt) {
         FineScope fs(h, Timers::F_BWD_WARP);
-        k_bwd_warp<32, false><<<nblk(b1.cnt, WPB), WPB * 32, (size_t)WPB * (b1.maxnf + 32 + 32 * BT_LD) * sizeof(double), s_warp>>>(
-            ds, h->d_sdesc.p + b1.off, b1.cnt, b1.maxnf, h->d_L.p, h->d_Dinv.p, h->d_y.p);
+        PICK(R, (k_bwd_warp<32, false>), (k_bwd_warp_multi<32, R>))<<<nblk(b1.cnt, WPB), WPB * 32, bwd_warp_smem(b1.maxnf, 32, R), s_warp>>>(
+            ds, h->d_sdesc.p + b1.off, b1.cnt, b1.maxnf, h->d_L.p, h->d_Dinv.p, V.y);
         LAUNCH(h);
     }
     const Batch& b5 = P.solve[5];
     if (b5.cnt) {
         FineScope fs(h, Timers::F_BWD_WARP);
-        if (h->merged_rows) k_bwd_warp<16, true><<<nblk(b5.cnt, WPB), WPB * 32, (size_t)WPB * (b5.maxnf + 32 + 32 * 17) * sizeof(double), s_warp>>>(
-            ds, h->d_sdesc.p + b5.off, b5.cnt, b5.maxnf, h->d_L.p, h->d_Dinv.p, h->d_y.p);
-        else k_bwd_warp<16, false><<<nblk(b5.cnt, WPB), WPB * 32, (size_t)WPB * (b5.maxnf + 32 + 32 * 17) * sizeof(double), s_warp>>>(
-            ds, h->d_sdesc.p + b5.off, b5.cnt, b5.maxnf, h->d_L.p, h->d_Dinv.p, h->d_y.p);
+        auto k = R > 1 ? PICK(R, (k_bwd_warp<16, true>), (k_bwd_warp_multi<16, R>))
+                       : h->merged_rows ? k_bwd_warp<16, true> : k_bwd_warp<16, false>;
+        k<<<nblk(b5.cnt, WPB), WPB * 32, bwd_warp_smem(b5.maxnf, 16, R), s_warp>>>(
+            ds, h->d_sdesc.p + b5.off, b5.cnt, b5.maxnf, h->d_L.p, h->d_Dinv.p, V.y);
         LAUNCH(h);
     }
     const Batch& b0 = P.solve[0];
     if (b0.cnt) {
         { FineScope fs(h, Timers::F_BWD_LEAF);
-        k_bwd_leaf<<<nblk(b0.cnt, 128), 128, 0, s_leaf>>>(ds, h->d_batches.p + b0.off, b0.cnt, h->d_L.p,
-                                                             h->d_Dinv.p, h->d_y.p);
+        PICK(R, k_bwd_leaf, k_bwd_leaf_multi<R>)<<<nblk(b0.cnt, 128), 128, 0, s_leaf>>>(ds, h->d_batches.p + b0.off, b0.cnt, h->d_L.p,
+                                                             h->d_Dinv.p, V.y);
         LAUNCH(h);
         }
     }
@@ -698,6 +717,7 @@ int build_plans(cb200_handle* h) {
     CUDA_OK(h->d_bigwork.upload(work, s));
     CUDA_OK(h->d_bigsync.alloc((size_t)nsync));
     CUDA_OK(h->d_partial.alloc((size_t)pmax));
+    h->partial_len = pmax;
     CUDA_OK(cudaStreamSynchronize(s));
     return 0;
 }
@@ -958,22 +978,23 @@ SubTrees subtrees(cb200_handle* h) {
 size_t subtree_smem_fwd(const cb200_handle* h) { return ((size_t)h->sub_maxcols + h->sub_maxrows + 8 * SUB_MAXNF) * sizeof(double); }
 size_t subtree_smem_bwd(const cb200_handle* h) { return ((size_t)h->sub_maxcols + 8 * (SUB_MAXNF + 32 * BT_LD)) * sizeof(double); }
 
-int sweeps_body(cb200_handle* h) {
+template <int R>
+int sweeps_body(cb200_handle* h, const SweepBufs& V) {
     const auto& S = h->S;
     // tickets and ready flags of the big-solve chains start from zero in every sweep (a memset node
     // of the captured graph); the error word [0] is reset per solve call
     if (h->d_bigsync.n > 1)
         CUDA_OK(cudaMemsetAsync(h->d_bigsync.p + 1, 0, (h->d_bigsync.n - 1) * sizeof(unsigned), h->stream));
-    if (h->nsub) {        // the bottom subtrees first: everything above them depends on their contributions
+    if (R == 1 && h->nsub) {  // the bottom subtrees first: everything above them depends on their contributions
         FineScope fs(h, Timers::F_FWD_SUB);
-        k_fwd_subtree<<<h->nsub, 256, subtree_smem_fwd(h), h->stream>>>(devsym(h), subtrees(h), h->d_L.p, h->d_y.p, h->d_uvec.p);
+        k_fwd_subtree<<<h->nsub, 256, subtree_smem_fwd(h), h->stream>>>(devsym(h), subtrees(h), h->d_L.p, V.y, V.uvec);
         LAUNCH(h);
     }
-    for (int lv = 0; lv < S.nlevels; ++lv) launch_fwd_level(h, h->plan[lv], lv);
-    for (int lv = S.nlevels - 1; lv >= 0; --lv) launch_bwd_level(h, h->plan[lv]);
-    if (h->nsub) {
+    for (int lv = 0; lv < S.nlevels; ++lv) launch_fwd_level<R>(h, h->plan[lv], lv, V);
+    for (int lv = S.nlevels - 1; lv >= 0; --lv) launch_bwd_level<R>(h, h->plan[lv], V);
+    if (R == 1 && h->nsub) {
         FineScope fs(h, Timers::F_BWD_SUB);
-        k_bwd_subtree<<<h->nsub, 256, subtree_smem_bwd(h), h->stream>>>(devsym(h), subtrees(h), h->d_L.p, h->d_Dinv.p, h->d_y.p);
+        k_bwd_subtree<<<h->nsub, 256, subtree_smem_bwd(h), h->stream>>>(devsym(h), subtrees(h), h->d_L.p, h->d_Dinv.p, V.y);
         LAUNCH(h);
     }
     CUDA_OK(cudaGetLastError());
@@ -991,7 +1012,8 @@ int tri_solve(cb200_handle* h, const double* d_rhs, double* d_sol) {
             k_mask_vec<<<nblk(h->N, 256), 256, 0, st>>>(h->d_y.p, h->d_topcolkeep.p, h->N); LAUNCH(h);
         }
     }
-    int rc = run_captured(h, h->g_solve, [&]() { return sweeps_body(h); });
+    const SweepBufs V{h->d_y.p, h->d_uvec.p, h->d_partial.p};
+    int rc = run_captured(h, h->g_solve, [&]() { return sweeps_body<1>(h, V); });
     if (rc) return rc;
     if (h->dist && h->N) {
         // every rank holds the solution on its own subtrees (+ the replicated top part): gather by
@@ -1058,6 +1080,194 @@ int read_scalars(cb200_handle* h, double* out, int first, int count) {
     return 0;
 }
 
+
+// ---- multi-right-hand-side sweeps (kernels_multi.cuh)
+constexpr size_t kMaxDynSmem = 200 * 1024;     // leaves room for the kernels' static shared memory (227 KB per CTA)
+
+template <int R> void set_multi_smem_attrs() {
+    for (const void* k : {(const void*)k_fwd_warp_multi<32, R>, (const void*)k_fwd_warp_multi<16, R>,
+                          (const void*)k_bwd_warp_multi<32, R>, (const void*)k_bwd_warp_multi<16, R>,
+                          (const void*)k_fwd_cta_multi<R>, (const void*)k_bwd_cta_multi<R>})
+        cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem);
+}
+
+// Allocates the multi-RHS buffers on the first multi call.  The sweep width is 4 unless the shared memory
+// of some warp- or CTA-class batch would not fit at that width (fronts of more than ~7000 rows solved by
+// one CTA); it is then 2, or 1.
+int ensure_multi(cb200_handle* h) {
+    if (h->multi_w) return 0;
+    auto fits = [&](int R) {
+        for (const LevelPlan& P : h->plan) {
+            const Batch &b1 = P.solve[1], &b5 = P.solve[5], &b2 = P.solve[2];
+            if (b1.cnt && (fwd_warp_smem(b1.maxnf, R) > kMaxDynSmem || bwd_warp_smem(b1.maxnf, 32, R) > kMaxDynSmem)) return false;
+            if (b5.cnt && (fwd_warp_smem(b5.maxnf, R) > kMaxDynSmem || bwd_warp_smem(b5.maxnf, 16, R) > kMaxDynSmem)) return false;
+            if (b2.cnt && ((size_t)b2.maxnf * R * sizeof(double) > kMaxDynSmem || bwd_cta_smem(b2.maxnf, R) > kMaxDynSmem)) return false;
+        }
+        return true;
+    };
+    int w = 4;
+    while (w > 1 && !fits(w)) w /= 2;
+    const size_t N = (size_t)std::max<int64_t>(1, h->N);
+    if (w > 1) {
+        CUDA_OK(h->d_my.alloc(N * w));
+        CUDA_OK(h->d_muvec.alloc(std::max<size_t>(1, h->S.rows.size()) * w));
+        CUDA_OK(h->d_mpartial.alloc((size_t)h->partial_len * w));
+        set_multi_smem_attrs<2>();
+        if (w == 4) set_multi_smem_attrs<4>();
+        CUDA_OK(cudaGetLastError());
+    }
+    for (DevBuf<double>* b : {&h->d_mb, &h->d_mx, &h->d_mdx, &h->d_me, &h->d_mstage}) {
+        CUDA_OK(b->alloc(N * w));
+        CUDA_OK(cudaMemsetAsync(b->p, 0, N * w * sizeof(double), h->stream));
+    }
+    CUDA_OK(h->d_mscal.alloc(8));
+    h->multi_w = w;
+    return 0;
+}
+
+// width of the next sweep for `rem` remaining columns: the full width, else the narrowest instantiated
+// width that holds them (a short chunk carries zero padding columns)
+int chunk_width(int w, int rem) {
+    if (rem >= w) return w;
+    return rem == 1 ? 1 : (rem == 2 ? 2 : 4);
+}
+
+// one R-wide sweep: column r < k of src (element i at src[i*rs + r*cs]) -> the same place of dst
+int tri_solve_multi(cb200_handle* h, int R, int k, const double* src, int64_t rs, int64_t cs,
+                    double* dst, int64_t drs, int64_t dcs) {
+    cudaStream_t st = h->stream;
+    const int64_t N = h->N;
+    double* y = R == 1 ? h->d_y.p : h->d_my.p;
+    h->tm.begin(Timers::SOLVE, st);
+    {
+        FineScope fs(h, Timers::F_PERMUTE);
+        k_pack_perm_multi<<<nblk(N * R, 256), 256, 0, st>>>(src, rs, cs, k, R, h->d_perm.p, N, y); LAUNCH(h);
+    }
+    int rc;
+    if (R == 1) {
+        const SweepBufs V{h->d_y.p, h->d_uvec.p, h->d_partial.p};
+        rc = run_captured(h, h->g_solve, [&]() { return sweeps_body<1>(h, V); });
+    } else if (R == 2) {
+        const SweepBufs V{h->d_my.p, h->d_muvec.p, h->d_mpartial.p};
+        rc = run_captured(h, h->g_msolve[0], [&]() { return sweeps_body<2>(h, V); });
+    } else {
+        const SweepBufs V{h->d_my.p, h->d_muvec.p, h->d_mpartial.p};
+        rc = run_captured(h, h->g_msolve[1], [&]() { return sweeps_body<4>(h, V); });
+    }
+    if (rc) return rc;
+    {
+        FineScope fs(h, Timers::F_PERMUTE);
+        k_unpack_perm_multi<<<nblk(N * R, 256), 256, 0, st>>>(y, k, R, h->d_perm.p, N, dst, drs, dcs); LAUNCH(h);
+    }
+    h->tm.end(st);
+    h->tm.nsolve += 1;
+    h->n_multi_sweeps += 1;
+    CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+template <int R>
+void launch_residual_multi(cb200_handle* h, const double* xi, double* e, unsigned long long* norms) {
+    cudaStream_t st = h->stream;
+    const double mean_row = 2.0 * (double)h->nnzK / (double)h->N;
+    if (mean_row > 48.0)
+        k_residual_multi<32, R><<<nblk(h->N * 32, 256), 256, 0, st>>>(h->N, h->d_cp.p, h->d_ri.p, h->d_nz.p, h->d_tp.p,
+                                                                      h->d_tc.p, h->d_tpos.p, xi, h->d_mb.p, e, norms);
+    else
+        k_residual_multi<4, R><<<nblk(h->N * 4, 256), 256, 0, st>>>(h->N, h->d_cp.p, h->d_ri.p, h->d_nz.p, h->d_tp.p,
+                                                                    h->d_tc.p, h->d_tpos.p, xi, h->d_mb.p, e, norms);
+    LAUNCH(h);
+    if (h->n_long_rows) {
+        k_residual_long_multi<R><<<h->n_long_rows, 256, 0, st>>>(h->d_long_rows.p, h->d_cp.p, h->d_ri.p, h->d_nz.p,
+                                                                 h->d_tp.p, h->d_tc.p, h->d_tpos.p, xi, h->d_mb.p, e, norms);
+        LAUNCH(h);
+    }
+}
+// e = b - K xi for R interleaved columns (b = d_mb); the norms go to d_mscal[4, 4 + R)
+int residual_multi(cb200_handle* h, int R, const double* xi, double* e) {
+    cudaStream_t st = h->stream;
+    h->tm.begin(Timers::SPMV, st);
+    CUDA_OK(cudaMemsetAsync(h->d_mscal.p + 4, 0, 4 * sizeof(unsigned long long), st));
+    if (R == 1) launch_residual_multi<1>(h, xi, e, h->d_mscal.p + 4);
+    else if (R == 2) launch_residual_multi<2>(h, xi, e, h->d_mscal.p + 4);
+    else launch_residual_multi<4>(h, xi, e, h->d_mscal.p + 4);
+    h->tm.end(st);
+    return 0;
+}
+// max |v_r| of R interleaved columns into d_mscal[slot, slot + R)
+int absmax_multi(cb200_handle* h, int R, const double* v, int slot) {
+    cudaStream_t st = h->stream;
+    CUDA_OK(cudaMemsetAsync(h->d_mscal.p + slot, 0, 4 * sizeof(unsigned long long), st));
+    const int g = std::min(nblk(h->N, 256), h->reduce_blocks);
+    if (R == 1) k_absmax_multi<1><<<g, 256, 0, st>>>(v, h->N, h->d_mscal.p + slot);
+    else if (R == 2) k_absmax_multi<2><<<g, 256, 0, st>>>(v, h->N, h->d_mscal.p + slot);
+    else k_absmax_multi<4><<<g, 256, 0, st>>>(v, h->N, h->d_mscal.p + slot);
+    LAUNCH(h);
+    return 0;
+}
+int read_mscal(cb200_handle* h, double* out, int first, int count) {
+    unsigned long long bits[8];
+    CUDA_OK(cudaMemcpyAsync(bits, h->d_mscal.p + first, count * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+    CUDA_OK(cudaStreamSynchronize(h->stream));
+    for (int i = 0; i < count; ++i) { long long b = (long long)bits[i]; std::memcpy(&out[i], &b, 8); }
+    return 0;
+}
+
+// Solution, refinement rounds and status of R interleaved systems (b in d_mb, k real columns), with the
+// per-column rules of cb200_solve_ir; the accepted iterates end in d_mx.
+int solve_ir_chunk(cb200_handle* h, int R, int k, int32_t* rounds, int32_t* okc) {
+    cudaStream_t st = h->stream;
+    const int64_t N = h->N;
+    const cb200_settings& S = h->st;
+    int rc = absmax_multi(h, R, h->d_mb.p, 0); if (rc) return rc;
+    rc = tri_solve_multi(h, R, R, h->d_mb.p, R, 1, h->d_mx.p, R, 1); if (rc) return rc;
+    for (int c = 0; c < k; ++c) { rounds[c] = 0; okc[c] = 1; }
+    if (!S.iterative_refinement_enable) {
+        rc = absmax_multi(h, R, h->d_mx.p, 4); if (rc) return rc;
+        double v[4];
+        rc = read_mscal(h, v, 4, R); if (rc) return rc;
+        for (int c = 0; c < k; ++c) okc[c] = std::isfinite(v[c]);
+        return 0;
+    }
+    // _iterative_refinement (kktsolver_directldl.jl:389-449), per column
+    rc = residual_multi(h, R, h->d_mx.p, h->d_me.p); if (rc) return rc;
+    double sc[8];
+    rc = read_mscal(h, sc, 0, 8); if (rc) return rc;
+    double normb[4], norme[4], last[4];
+    bool done[4];
+    for (int c = 0; c < R; ++c) {
+        normb[c] = sc[c]; norme[c] = sc[4 + c]; last[c] = 0;
+        done[c] = c >= k;
+        if (c < k && !std::isfinite(norme[c])) { okc[c] = 0; done[c] = true; }
+    }
+    for (int i = 0; i < S.iterative_refinement_max_iter; ++i) {
+        bool act[4], any = false;
+        for (int c = 0; c < R; ++c) {
+            if (!done[c] && norme[c] <= S.iterative_refinement_abstol + S.iterative_refinement_reltol * normb[c]) done[c] = true;
+            act[c] = !done[c]; any |= act[c];
+            if (act[c]) last[c] = norme[c];
+        }
+        if (!any) break;
+        rc = tri_solve_multi(h, R, R, h->d_me.p, R, 1, h->d_mdx.p, R, 1); if (rc) return rc;
+        k_axpy_multi<<<nblk(N * R, 256), 256, 0, st>>>(h->d_mdx.p, h->d_mx.p, N * R); LAUNCH(h);
+        rc = residual_multi(h, R, h->d_mdx.p, h->d_me.p); if (rc) return rc;
+        rc = read_mscal(h, sc, 4, R); if (rc) return rc;
+        unsigned take = 0;                         // columns whose new iterate replaces x (the single path's swap)
+        for (int c = 0; c < R; ++c) {
+            if (!act[c]) continue;
+            norme[c] = sc[c];
+            rounds[c]++;
+            if (!std::isfinite(norme[c])) { okc[c] = 0; done[c] = true; continue; }
+            const double ratio = last[c] / norme[c];
+            if (ratio < S.iterative_refinement_stop_ratio) {
+                if (ratio > 1.0) take |= 1u << c;
+                done[c] = true;
+            } else take |= 1u << c;
+        }
+        if (take) { k_select_cols<<<nblk(N * R, 256), 256, 0, st>>>(h->d_mx.p, h->d_mdx.p, N, R, take); LAUNCH(h); }
+    }
+    return 0;
+}
 }  // namespace
 
 extern "C" {
@@ -1230,7 +1440,7 @@ void cb200_destroy(cb200_handle* h) {
     if (h->stream) { cudaStreamSynchronize(h->stream); }
     // graphs captured with NCCL kernels inside hold references on the communicator: ncclCommDestroy waits
     // for them, so the executables go first (seen as a teardown hang with CB200_DIST_GRAPH=1)
-    for (GraphExec* g : {&h->g_factor[0], &h->g_factor[1], &h->g_solve})
+    for (GraphExec* g : {&h->g_factor[0], &h->g_factor[1], &h->g_solve, &h->g_msolve[0], &h->g_msolve[1]})
         if (g->exec) { cudaGraphExecDestroy(g->exec); g->exec = nullptr; }
     if (h->comm && g_nccl.ok) { g_nccl.CommDestroy(h->comm); h->comm = nullptr; }
     cudaStream_t s = h->stream;
@@ -1581,6 +1791,144 @@ int32_t cb200_solve_ir(cb200_handle* h, const double* rhsx, const double* rhsz,
     return ok ? 0 : 1;
 }
 
+int32_t cb200_solve_multi(cb200_handle* h, int32_t nrhs, double* X, int64_t ldx, const double* B, int64_t ldb) {
+    const int64_t N = h->N;
+    if (nrhs < 0) { set_error("cb200_solve_multi: nrhs < 0"); return -2; }
+    if (nrhs == 0) return 0;
+    if (!X || !B) { set_error("cb200_solve_multi: X or B is NULL"); return -2; }
+    if (ldx < N || ldb < N) { set_error("cb200_solve_multi: leading dimension < N"); return -2; }
+    if (N == 0) return 0;
+    CUDA_OK(cudaSetDevice(h->st.device));
+    int rc = ensure_multi(h); if (rc) return rc;
+    cudaStream_t st = h->stream;
+    if (h->dist || h->use_subtree) {
+        // column by column through cb200_solve (multi-GPU sweeps and the subtree kernels have no R-wide
+        // form); the last single solve (download selector 6) is kept
+        CUDA_OK(cudaMemcpyAsync(h->d_me.p, h->d_x.p, N * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        for (int32_t j = 0; j < nrhs && rc == 0; ++j) {
+            rc = cb200_solve(h, X + j * ldx, B + j * ldb);
+            h->n_percol += 1;
+        }
+        // put the last single solution back on every path, failed calls included
+        const cudaError_t e = cudaMemcpyAsync(h->d_x.p, h->d_me.p, N * sizeof(double), cudaMemcpyDeviceToDevice, st);
+        if (rc) return rc;
+        CUDA_OK(e);
+        CUDA_OK(cudaStreamSynchronize(st));
+        return 0;
+    }
+    rc = reset_chain_error(h); if (rc) return rc;
+    for (int32_t c0 = 0; c0 < nrhs;) {
+        const int R = chunk_width(h->multi_w, nrhs - c0), k = std::min(R, nrhs - c0);
+        CUDA_OK(cudaMemcpy2DAsync(h->d_mstage.p, N * sizeof(double), B + c0 * ldb, ldb * sizeof(double),
+                                  N * sizeof(double), k, cudaMemcpyHostToDevice, st));
+        rc = tri_solve_multi(h, R, k, h->d_mstage.p, 1, N, h->d_mstage.p, 1, N); if (rc) return rc;
+        CUDA_OK(cudaMemcpy2DAsync(X + c0 * ldx, ldx * sizeof(double), h->d_mstage.p, N * sizeof(double),
+                                  N * sizeof(double), k, cudaMemcpyDeviceToHost, st));
+        c0 += k;
+    }
+    unsigned chain_err = 0;
+    rc = read_chain_error(h, &chain_err); if (rc) return rc;
+    CUDA_OK(cudaStreamSynchronize(st));
+    h->tm.collect();
+    if (chain_err) { set_error("cb200_solve_multi: a big-front solve chain timed out waiting for a block"); return -4; }
+    return 0;
+}
+
+int32_t cb200_solve_ir_multi(cb200_handle* h, int32_t nrhs, const double* rhsx, const double* rhsz,
+                             double* lhsx, double* lhsz, int32_t* ir_rounds, int32_t* status) {
+    if (!h->maps_set) { set_error("cb200_solve_ir_multi: cb200_set_maps not called"); return -2; }
+    if (nrhs < 0) { set_error("cb200_solve_ir_multi: nrhs < 0"); return -2; }
+    if (nrhs == 0) return 0;
+    const int64_t N = h->N, n = h->n, m = h->m;
+    if ((n && !rhsx) || (m && !rhsz)) { set_error("cb200_solve_ir_multi: rhsx or rhsz is NULL"); return -2; }
+    for (int32_t j = 0; j < nrhs; ++j) { if (ir_rounds) ir_rounds[j] = 0; if (status) status[j] = 0; }
+    if (N == 0) return 0;
+    CUDA_OK(cudaSetDevice(h->st.device));
+    int rc = ensure_multi(h); if (rc) return rc;
+    cudaStream_t st = h->stream;
+    if ((int64_t)h->d_msol.n < N * nrhs) CUDA_OK(h->d_msol.alloc((size_t)(N * nrhs)));
+    h->msol_cols = nrhs;
+    std::vector<int32_t> rounds(nrhs, 0), okv(nrhs, 1);
+    if (h->dist || h->use_subtree) {
+        // column by column through cb200_solve_ir; what cb200_setrhs stored and the last single solution
+        // (download selector 6) are put back afterwards
+        CUDA_OK(cudaMemcpyAsync(h->d_me.p, h->d_x.p, N * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        if (n) CUDA_OK(cudaMemcpyAsync(h->d_mdx.p, h->d_rx.p, n * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        if (m) CUDA_OK(cudaMemcpyAsync(h->d_mdx.p + n, h->d_rz.p, m * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        for (int32_t j = 0; j < nrhs && rc >= 0; ++j) {
+            if (h->resident) {
+                if (n) CUDA_OK(cudaMemcpyAsync(h->d_rx.p, rhsx + j * n, n * sizeof(double), cudaMemcpyDeviceToDevice, st));
+                if (m) CUDA_OK(cudaMemcpyAsync(h->d_rz.p, rhsz + j * m, m * sizeof(double), cudaMemcpyDeviceToDevice, st));
+                rc = cb200_solve_ir(h, nullptr, nullptr, nullptr, nullptr, &rounds[j]);
+            } else {
+                rc = cb200_solve_ir(h, n ? rhsx + j * n : nullptr, m ? rhsz + j * m : nullptr,
+                                    lhsx ? lhsx + j * n : nullptr, lhsz ? lhsz + j * m : nullptr, &rounds[j]);
+            }
+            if (rc < 0) break;
+            okv[j] = rc == 0;
+            CUDA_OK(cudaMemcpyAsync(h->d_msol.p + j * N, h->d_x.p, N * sizeof(double), cudaMemcpyDeviceToDevice, st));
+            h->n_percol += 1;
+        }
+        // restore the single-RHS state on every path, failed calls included
+        cudaError_t e = cudaMemcpyAsync(h->d_x.p, h->d_me.p, N * sizeof(double), cudaMemcpyDeviceToDevice, st);
+        if (n && e == cudaSuccess) e = cudaMemcpyAsync(h->d_rx.p, h->d_mdx.p, n * sizeof(double), cudaMemcpyDeviceToDevice, st);
+        if (m && e == cudaSuccess) e = cudaMemcpyAsync(h->d_rz.p, h->d_mdx.p + n, m * sizeof(double), cudaMemcpyDeviceToDevice, st);
+        if (rc < 0) return rc;
+        CUDA_OK(e);
+        CUDA_OK(cudaStreamSynchronize(st));
+    } else {
+        const int w = h->multi_w;
+        if (!h->resident) {
+            if ((int64_t)h->d_mrx.n < std::max<int64_t>(1, n) * w) CUDA_OK(h->d_mrx.alloc((size_t)std::max<int64_t>(1, n) * w));
+            if ((int64_t)h->d_mrz.n < std::max<int64_t>(1, m) * w) CUDA_OK(h->d_mrz.alloc((size_t)std::max<int64_t>(1, m) * w));
+        }
+        rc = reset_chain_error(h); if (rc) return rc;
+        for (int32_t c0 = 0; c0 < nrhs;) {
+            const int R = chunk_width(w, nrhs - c0), k = std::min(R, nrhs - c0);
+            const double* rx = rhsx ? rhsx + c0 * n : nullptr;
+            const double* rz = rhsz ? rhsz + c0 * m : nullptr;
+            if (!h->resident) {         // host columns -> device staging (the caller may reuse them on return)
+                if (n) CUDA_OK(cudaMemcpyAsync(h->d_mrx.p, rx, k * n * sizeof(double), cudaMemcpyHostToDevice, st));
+                if (m) CUDA_OK(cudaMemcpyAsync(h->d_mrz.p, rz, k * m * sizeof(double), cudaMemcpyHostToDevice, st));
+                rx = h->d_mrx.p; rz = h->d_mrz.p;
+            }
+            k_build_rhs_multi<<<nblk(N * R, 256), 256, 0, st>>>(rx, rz, n, m, N, k, R, h->d_mb.p); LAUNCH(h);
+            rc = solve_ir_chunk(h, R, k, rounds.data() + c0, okv.data() + c0); if (rc) return rc;
+            k_deinterleave<<<nblk(N * R, 256), 256, 0, st>>>(h->d_mx.p, k, R, N, h->d_msol.p + c0 * N, N); LAUNCH(h);
+            c0 += k;
+        }
+        if (!h->resident) {
+            if (lhsx && n) CUDA_OK(cudaMemcpy2DAsync(lhsx, n * sizeof(double), h->d_msol.p, N * sizeof(double),
+                                                     n * sizeof(double), nrhs, cudaMemcpyDeviceToHost, st));
+            if (lhsz && m) CUDA_OK(cudaMemcpy2DAsync(lhsz, m * sizeof(double), h->d_msol.p + n, N * sizeof(double),
+                                                     m * sizeof(double), nrhs, cudaMemcpyDeviceToHost, st));
+        }
+        unsigned chain_err = 0;
+        rc = read_chain_error(h, &chain_err); if (rc) return rc;
+        CUDA_OK(cudaStreamSynchronize(st));
+        h->tm.collect();
+        if (chain_err) {
+            set_error("cb200_solve_ir_multi: a big-front solve chain timed out waiting for a block");
+            std::fill(okv.begin(), okv.end(), 0);
+        }
+        if (!h->resident) {            // failed columns are NaN-filled, as cb200_solve_ir does
+            const double qnan = std::numeric_limits<double>::quiet_NaN();
+            for (int32_t j = 0; j < nrhs; ++j) {
+                if (okv[j]) continue;
+                if (lhsx) std::fill(lhsx + j * n, lhsx + (j + 1) * n, qnan);
+                if (lhsz) std::fill(lhsz + j * m, lhsz + (j + 1) * m, qnan);
+            }
+        }
+    }
+    bool all_ok = true;
+    for (int32_t j = 0; j < nrhs; ++j) {
+        if (ir_rounds) ir_rounds[j] = rounds[j];
+        if (status) status[j] = okv[j] ? 0 : 1;
+        all_ok &= okv[j] != 0;
+    }
+    return all_ok ? 0 : 1;
+}
+
 static int32_t update_block(cb200_handle* h, const DevBuf<int64_t>& map, const double* values, int64_t len) {
     if (!h->maps_set) { set_error("cb200_update_P/A: cb200_set_maps not called"); return -2; }
     if ((int64_t)map.n != len) { set_error("cb200_update_P/A: length mismatch"); return -2; }
@@ -1613,6 +1961,7 @@ int32_t cb200_download(cb200_handle* h, int32_t what, double* out, int64_t len) 
                   CUDA_OK(cudaMemcpyAsync(&v, h->d_nreg.p, sizeof(v), cudaMemcpyDeviceToHost, st));
                   CUDA_OK(cudaStreamSynchronize(st)); out[0] = (double)v; return 0; }
         case 6: src = h->d_x.p; n = h->N; break;       // full solution [x; z; expansion variables] of the last solve
+        case 8: src = h->d_msol.p; n = h->N * h->msol_cols; break;   // the same, N x nrhs, of the last cb200_solve_ir_multi
         case 7: { if (len != 64) { set_error("download: length"); return -2; }     // ORIGINAL indices of the first 64 regularised pivots
                   int32_t v[64]; unsigned int cnt = 0;
                   CUDA_OK(cudaMemcpyAsync(v, h->d_reglog.p, sizeof(v), cudaMemcpyDeviceToHost, st));
@@ -1679,7 +2028,7 @@ int32_t cb200_dist_init(cb200_handle* h, int32_t rank, int32_t nranks, const cha
         if (!rc) rc = upload_tile_lists(h);
         if (rc) return rc;
         // the captured launch sequences (if any) belong to the single-GPU plans
-        for (GraphExec* g : {&h->g_factor[0], &h->g_factor[1], &h->g_solve}) {
+        for (GraphExec* g : {&h->g_factor[0], &h->g_factor[1], &h->g_solve, &h->g_msolve[0], &h->g_msolve[1]}) {
             if (g->exec) { cudaGraphExecDestroy(g->exec); g->exec = nullptr; }
             g->failed = false;
         }
@@ -1722,13 +2071,14 @@ int32_t cb200_get_stats(const cb200_handle* h, double* out, int32_t len) {
         }
         if (nf * ns >= 65536 && ns > 32) big_bytes += 8.0 * nf * ns;
     }
-    double v[21] = {S.flops, schur, panel_large - schur, (double)S.nnzL, (double)S.nlevels, (double)S.nsuper,
+    double v[23] = {S.flops, schur, panel_large - schur, (double)S.nnzL, (double)S.nlevels, (double)S.nsuper,
                     nlarge, big_bytes, (double)S.upd_total * 8.0, (double)S.panel_off.back() * 8.0,
                     (double)S.ordering_used, my_flops, h->use_tma ? 1.0 : 0.0, (double)h->tma_kmajor,
                     (double)((h->g_factor[0].exec != nullptr) + (h->g_factor[1].exec != nullptr)),
                     h->g_solve.exec ? 1.0 : 0.0, (double)h->nsub,
-                    (double)h->n_schur_tiles, (double)h->n_schur_rects, (double)h->n_asm_tiles, (double)h->n_asm_rects};
-    for (int i = 0; i < len && i < 21; ++i) out[i] = v[i];
+                    (double)h->n_schur_tiles, (double)h->n_schur_rects, (double)h->n_asm_tiles, (double)h->n_asm_rects,
+                    h->n_multi_sweeps, h->n_percol};
+    for (int i = 0; i < len && i < 23; ++i) out[i] = v[i];
     return 0;
 }
 

@@ -10,7 +10,8 @@
 //   G6  extend-add                        fused in G4 ; k_assemble_tiles ; add_tile_rects (also in the Schur
 //                                         epilogue) ; k_assemble_atomic
 //   G7  multifrontal triangular solves    k_fwd_{leaf,warp<16|32>,cta}, k_bwd_*, k_big_{asm,tri,gemv}_*, k_*_subtree,
-//                                         k_pack_perm, k_unpack_perm
+//                                         k_pack_perm, k_unpack_perm ; R-wide forms for several right-hand sides:
+//                                         kernels_multi.cuh
 //   G8  symmetric SpMV residual + norm    k_residual, k_residual_long
 //   G9  multi-GPU helpers                 k_zero_panels, k_mask_vec  (collectives: api_cuda.cu)
 #pragma once
@@ -1620,8 +1621,11 @@ k_fwd_cta(DevSym S, const SolveDesc* __restrict__ desc, const double* __restrict
             part[qd][i] = acc;
         }
         __syncthreads();
-        if (tid < sb) {
-            const double x = w[kb + tid] + part[0][tid] + part[1][tid] + part[2][tid] + part[3][tid];
+        if (tid < SB) {
+            // zero beyond sb: row_dot64 multiplies the whole 64-entry window (its L loads are zero there), and
+            // 0 * uninitialised shared memory is NaN when those bits happen to be a NaN or an infinity
+            double x = 0.0;
+            if (tid < sb) x = w[kb + tid] + part[0][tid] + part[1][tid] + part[2][tid] + part[3][tid];
             xs[tid] = x;
         }
         __syncthreads();

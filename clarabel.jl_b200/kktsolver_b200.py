@@ -82,6 +82,13 @@ class B200DirectLDLSolver:
         assert x.dtype == np.float64 and x.flags.c_contiguous
         _lib.check(self._L.cb200_solve(self._h, _p(x), _p(bb)), "cb200_solve")
 
+    def solve_multi(self, X, B):
+        """cb200_solve_multi: X[:, j] = K^-1 B[:, j] for every column of the N x k arrays, one pass over L per
+        sweep of up to 4 columns.  Both arrays in Fortran (column-major) order; X is written in place."""
+        B = np.asfortranarray(B, dtype=np.float64)
+        assert X.dtype == np.float64 and X.flags.f_contiguous and X.shape == B.shape and B.shape[0] == self.N
+        _lib.check(self._L.cb200_solve_multi(self._h, B.shape[1], _p(X), self.N, _p(B), self.N), "cb200_solve_multi")
+
     def info(self):
         a, l, g = C.c_int64(), C.c_int64(), C.c_int32()
         self._L.cb200_info(self._h, C.byref(a), C.byref(l), C.byref(g))
@@ -113,11 +120,12 @@ class B200DirectLDLSolver:
         return {self._L.cb200_fine_timer_name(i).decode(): float(out[i]) for i in range(n)}
 
     def stats(self):
-        out = np.zeros(21)
-        self._L.cb200_get_stats(self._h, _p(out), 21)
+        out = np.zeros(23)
+        self._L.cb200_get_stats(self._h, _p(out), 23)
         keys = ["flops", "schur_flops", "panel_flops", "nnzL", "nlevels", "nsuper", "nlarge",
                 "big_solve_bytes", "upd_bytes", "panel_bytes", "ordering_used", "rank_flops", "use_tma", "tma_kmajor",
-                "factor_graphs", "solve_graph", "subtrees", "schur_tiles", "schur_rects", "asm_tiles", "asm_rects"]
+                "factor_graphs", "solve_graph", "subtrees", "schur_tiles", "schur_rects", "asm_tiles", "asm_rects",
+                "multi_sweeps", "multi_percol"]
         return dict(zip(keys, out.tolist()))
 
     def reset_timers(self):
@@ -257,6 +265,35 @@ class B200KKTSolver:
                         "cb200_solve_ir")
         self.ir_rounds += rounds.value; self.n_solves += 1
         return ok
+
+    def solve_multi(self, rhsx, rhsz, lhsx=None, lhsz=None):
+        """setrhs + solve for k systems at once (cb200_solve_ir_multi): rhsx n x k, rhsz m x k, lhsx / lhsz the
+        same shapes or None.  The arrays are column-major: Fortran order, or the transpose of a C-order
+        k x n array.  Column j equals setrhs(rhsx[:, j], rhsz[:, j]) + solve bit for bit, with the same
+        refinement rounds.  Returns (ok[k], ir_rounds[k]); a failed column's lhs is NaN.  Leaves what
+        setrhs stored untouched."""
+        rx = np.asfortranarray(rhsx, dtype=np.float64); rz = np.asfortranarray(rhsz, dtype=np.float64)
+        k = rx.shape[1]
+        assert rx.shape == (self.n, k) and rz.shape == (self.m, k)
+        for a, n in ((lhsx, self.n), (lhsz, self.m)):
+            if a is not None:
+                assert a.dtype == np.float64 and a.flags.f_contiguous and a.shape == (n, k)
+        rounds = np.zeros(k, dtype=np.int32); status = np.zeros(k, dtype=np.int32)
+        _lib.check(self.ldl._L.cb200_solve_ir_multi(self.ldl._h, k, _p(rx), _p(rz), _p(lhsx), _p(lhsz),
+                                                     _p(rounds), _p(status)), "cb200_solve_ir_multi")
+        self.ir_rounds += int(rounds.sum()); self.n_solves += k
+        return status == 0, rounds
+
+    def solve_multi_staged(self, px, pz, k):
+        """Resident mode: solve_multi from device addresses of the column-major n x k / m x k right-hand sides;
+        the solutions stay on the device (download selector 8, N x k).  Returns (ok[k], ir_rounds[k])."""
+        assert self.ldl.resident
+        rounds = np.zeros(k, dtype=np.int32); status = np.zeros(k, dtype=np.int32)
+        _lib.check(self.ldl._L.cb200_solve_ir_multi(self.ldl._h, int(k), C.c_void_p(px) if px else None,
+                                                     C.c_void_p(pz) if pz else None, None, None,
+                                                     _p(rounds), _p(status)), "cb200_solve_ir_multi")
+        self.ir_rounds += int(rounds.sum()); self.n_solves += int(k)
+        return status == 0, rounds
 
     def update_P(self, P):
         v = _c64(P.data)

@@ -17,8 +17,8 @@ EXPORTED = [
     "cb200_symbolic_stat", "cb200_symbolic_flops", "cb200_symbolic_get", "cb200_symbolic_tile_lists",
     "cb200_order_amd", "cb200_order_nd",
     "cb200_create", "cb200_destroy", "cb200_update_values", "cb200_scale_values",
-    "cb200_refactor", "cb200_solve", "cb200_info",
-    "cb200_set_maps", "cb200_update_cones", "cb200_setrhs", "cb200_solve_ir", "cb200_update_P", "cb200_update_A",
+    "cb200_refactor", "cb200_solve", "cb200_solve_multi", "cb200_info",
+    "cb200_set_maps", "cb200_update_cones", "cb200_setrhs", "cb200_solve_ir", "cb200_solve_ir_multi", "cb200_update_P", "cb200_update_A",
     "cb200_download", "cb200_get_timers", "cb200_reset_timers", "cb200_last_error",
     "cb200_get_stream", "cb200_set_resident",
     "cb200_symbolic_partition", "cb200_nccl_unique_id", "cb200_dist_init",
@@ -69,11 +69,13 @@ def lib():
         L.cb200_scale_values.argtypes = [P, P, I64, D]; L.cb200_scale_values.restype = I32
         L.cb200_refactor.argtypes = [P]; L.cb200_refactor.restype = I32
         L.cb200_solve.argtypes = [P, P, P]; L.cb200_solve.restype = I32
+        L.cb200_solve_multi.argtypes = [P, I32, P, I64, P, I64]; L.cb200_solve_multi.restype = I32
         L.cb200_info.argtypes = [P, P, P, P]; L.cb200_info.restype = I32
         L.cb200_set_maps.argtypes = [P, I64, I64, I64, P, I64, P, I64, P, I64, P, I64, P, P, P, P, P]
         L.cb200_set_maps.restype = I32
         L.cb200_update_cones.argtypes = [P] * 7; L.cb200_update_cones.restype = I32
         L.cb200_solve_ir.argtypes = [P] * 6; L.cb200_solve_ir.restype = I32
+        L.cb200_solve_ir_multi.argtypes = [P, I32] + [P] * 6; L.cb200_solve_ir_multi.restype = I32
         L.cb200_setrhs.argtypes = [P, P, P]; L.cb200_setrhs.restype = I32
         L.cb200_update_P.argtypes = [P, P, I64]; L.cb200_update_P.restype = I32
         L.cb200_update_A.argtypes = [P, P, I64]; L.cb200_update_A.restype = I32

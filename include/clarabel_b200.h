@@ -147,6 +147,25 @@ int32_t cb200_setrhs(cb200_handle* h, const double* rhsx, const double* rhsz);
  * rhsx == rhsz == NULL: use the right-hand side set by cb200_setrhs. */
 int32_t cb200_solve_ir(cb200_handle* h, const double* rhsx, const double* rhsz,
                        double* lhsx, double* lhsz, int32_t* ir_rounds);
+/* Several right-hand sides against the current factorisation, one pass over L per sweep: a sweep carries up
+ * to 4 columns (more columns run in ceil(nrhs / 4) sweeps), interleaved so that every L entry is loaded once
+ * for all of them.  These calls leave the single-RHS state alone: what cb200_setrhs stored and the last
+ * single solution (download selector 6) are unchanged.  nrhs == 0 is a no-op; nrhs < 0, a leading
+ * dimension < N or a NULL required pointer return -2.
+ * cb200_solve_multi: B, X column-major N x nrhs with leading dimensions ldb, ldx >= N (host pointers, like
+ * cb200_solve).  Column j of X is bit-for-bit what cb200_solve(h, x, B[:, j]) returns. */
+int32_t cb200_solve_multi(cb200_handle* h, int32_t nrhs, double* X, int64_t ldx,
+                          const double* B, int64_t ldb);
+/* kktsolver_setrhs! + kktsolver_solve! for nrhs systems: rhsx n x nrhs, rhsz m x nrhs (column-major, packed),
+ * lhsx / lhsz the same shapes or NULL.  Iterative refinement runs per column with the single-RHS rules
+ * (kktsolver_directldl.jl:389-449).  ir_rounds[nrhs] and status[nrhs] (0 ok, 1 numerical failure) are
+ * optional outputs.  Returns 0 if every column succeeded, 1 otherwise; failed columns of lhsx / lhsz are
+ * NaN-filled as in cb200_solve_ir.  Column j is bit-for-bit what cb200_solve_ir(h, rhsx[:, j], rhsz[:, j], ...)
+ * returns, with the same ir_rounds.  Needs cb200_set_maps.  Resident mode: rhsx / rhsz are device pointers
+ * and the results stay on the device (cb200_download selector 8).  In multi-GPU mode and with
+ * CB200_SUBTREE=1 both calls solve column by column through the single-RHS path (cb200_get_stats 22). */
+int32_t cb200_solve_ir_multi(cb200_handle* h, int32_t nrhs, const double* rhsx, const double* rhsz,
+                             double* lhsx, double* lhsz, int32_t* ir_rounds, int32_t* status);
 /* kktsolver_update_P!/A! — kktsolver_directldl.jl:374-386 */
 int32_t cb200_update_P(cb200_handle* h, const double* values, int64_t len);
 int32_t cb200_update_A(cb200_handle* h, const double* values, int64_t len);
@@ -155,10 +174,12 @@ int32_t cb200_update_A(cb200_handle* h, const double* values, int64_t len);
  * what: 0 device KKT nzval (unregularised, len nnzK), 1 D (permuted, len N), 2 panel storage,
  *       3 perm (as doubles), 4 last static regulariser (len 1), 5 regularised-pivot count (len 1),
  *       6 full solution [x; z; expansion variables] of the last solve (len N),
- *       7 original indices of the first 64 dynamically regularised pivots of the last factorisation (len 64, -1 = none) */
+ *       7 original indices of the first 64 dynamically regularised pivots of the last factorisation (len 64, -1 = none),
+ *       8 full solutions of the last cb200_solve_ir_multi, N x nrhs column-major (len N * nrhs) */
 int32_t cb200_download(cb200_handle* h, int32_t what, double* out, int64_t len);
 /* timers (ms, accumulated CUDA-event times on the handle's stream): 0 cone update + scatter,
- * 1 factor, 2 triangular solves, 3 spmv/residual ; counters: 4 #factor, 5 #solves, 6 #kernel launches ;
+ * 1 factor, 2 triangular solves, 3 spmv/residual ; counters: 4 #factor, 5 #solve sweeps (a multi-RHS sweep of
+ * up to 4 columns counts once), 6 #kernel launches ;
  * with cb200_set_detail(h,1) also per kernel class inside the factorisation: 7 k_schur_large,
  * 8 pivot-block phase (k_diag64 + k_rows64), 9 small fronts (k_factor_small), 10 assembly */
 int32_t cb200_get_timers(cb200_handle* h, double* out, int32_t len);
@@ -177,7 +198,8 @@ const char* cb200_fine_timer_name(int32_t i);
  * 10 ordering used, 11 flops of this rank's fronts, 12 TMA tensor maps in use, 13 their k-major order,
  * 14 factorisation graphs instantiated (0-2), 15 solve-sweep graph instantiated, 16 bottom subtrees
  * solved by k_fwd_subtree / k_bwd_subtree, 17 Schur tiles and 18 their child rectangles, 19 assembly
- * tiles and 20 their child rectangles (all large batches, cb200_symbolic_tile_lists) */
+ * tiles and 20 their child rectangles (all large batches, cb200_symbolic_tile_lists), 21 multi-RHS sweeps run
+ * batched, 22 columns of the multi-RHS calls solved one by one through the single-RHS path */
 int32_t cb200_get_stats(const cb200_handle* h, double* out, int32_t len);
 /* ---------------------------------------------------------------- multi-GPU (one process per GPU)
  * Every rank creates the same handle on its own device (replicated symbolic analysis), then
