@@ -6,6 +6,7 @@
 #include "api_common.h"
 #include "kernels.cuh"
 #include "kernels_multi.cuh"
+#include "kernels_scaling.cuh"
 
 #include <dlfcn.h>
 #include <nccl.h>
@@ -296,6 +297,19 @@ struct cb200_handle {
     GraphExec g_msolve[2];                          // sweep graphs of width 2 and 4 (width 1 is g_solve)
     int64_t partial_len = 1;                        // doubles of d_partial (one column)
     double n_multi_sweeps = 0, n_percol = 0;        // cb200_get_stats 21 / 22
+    // device NT scaling (cb200_update_scaling, G10): tables and outputs built by the first call
+    std::vector<int32_t> h_ctype; std::vector<int64_t> h_cdim;      // the cone table of cb200_set_maps
+    bool scale_ready = false;
+    int64_t nnn = 0, psd_ltotal = 0;
+    int32_t nsoc_warp = 0, nsoc_cta = 0, npsd_smem = 0, npsd_glob = 0;
+    size_t psd_smem_bytes = 0;                                      // dynamic shared memory of k_scale_psd<true>
+    DevBuf<int32_t> d_nn_rows;                                      // m-space rows of the NN cones
+    DevBuf<int32_t> d_soc_list, d_soc_dim; DevBuf<int64_t> d_soc_moff, d_soc_srow;   // list: warp class, then CTA class
+    DevBuf<int32_t> d_psd_list; DevBuf<int64_t> d_psd_moff, d_psd_loff, d_psd_woff;  // list: shared-memory, then global
+    DevBuf<double> d_lam, d_psd_Rinv, d_psd_lam, d_psd_ws, d_ss, d_sz;
+    DevBuf<int> d_scale_flags;                                      // [0] failure, [1] max Jacobi sweeps
+    cudaEvent_t ev_scale[2] = {nullptr, nullptr};
+    double scale_ms = 0, last_sweeps = 0;                           // cb200_get_timers 11, cb200_get_stats 25
 };
 
 namespace {
@@ -1449,6 +1463,7 @@ void cb200_destroy(cb200_handle* h) {
         if (h->ev_join[i]) cudaEventDestroy(h->ev_join[i]);
     }
     if (h->ev_fork) cudaEventDestroy(h->ev_fork);
+    for (cudaEvent_t e : h->ev_scale) if (e) cudaEventDestroy(e);
     delete h;
     if (s) cudaStreamDestroy(s);
 }
@@ -1650,6 +1665,8 @@ int32_t cb200_set_maps(cb200_handle* h, int64_t n, int64_t m, int64_t p,
         CUDA_OK(h->d_rx.alloc(std::max<int64_t>(1, n))); CUDA_OK(h->d_rz.alloc(std::max<int64_t>(1, m)));
         if (h->psd_maxn) CUDA_OK(cudaFuncSetAttribute(k_psd_skron, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                       std::max(48 * 1024, h->psd_maxn * h->psd_maxn * 8)));
+        h->h_ctype.assign(cone_type, cone_type + ncones); h->h_cdim.assign(cone_dim, cone_dim + ncones);
+        h->scale_ready = false;
         CUDA_OK(cudaStreamSynchronize(s));
         h->maps_set = true;
         return 0;
@@ -1664,10 +1681,11 @@ int32_t cb200_update_cones(cb200_handle* h, const double* w, const double* soc_e
     cudaStream_t st = h->stream;
     h->tm.begin(Timers::CONE, st);
     // host pointers normally; in resident mode (cb200_set_resident) non-NULL arguments are DEVICE pointers
-    // (inputs staged in HBM by the caller, copied device-to-device) and NULL keeps the previous state
+    // (inputs staged in HBM by the caller, copied device-to-device).  In both modes NULL keeps the state on the
+    // device: what the previous call uploaded, or what cb200_update_scaling computed.
     const cudaMemcpyKind kind = h->resident ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     auto put = [&](double* dst, const double* src, int64_t len) -> cudaError_t {
-        if (len <= 0 || (h->resident && !src)) return cudaSuccess;
+        if (len <= 0 || !src) return cudaSuccess;
         return cudaMemcpyAsync(dst, src, len * sizeof(double), kind, st);
     };
     CUDA_OK(put(h->d_w.p, w, h->m));
@@ -1703,6 +1721,155 @@ int32_t cb200_update_cones(cb200_handle* h, const double* w, const double* soc_e
     int rc = factor(h, /*static_reg=*/true);
     if (rc) return rc;
     return finish_factor(h);
+}
+
+// G10 tables and output buffers, built by the first cb200_update_scaling / cb200_get_scaling from the cone table of
+// cb200_set_maps, so that a caller that keeps the host scaling pays no memory for them.
+static int prepare_scaling(cb200_handle* h) {
+    if (h->scale_ready) return 0;
+    int optin = 0;
+    CUDA_OK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->st.device));
+    cudaFuncAttributes fa;
+    CUDA_OK(cudaFuncGetAttributes(&fa, k_scale_psd<true>));
+    const int64_t dyn_cap = (int64_t)optin - (int64_t)fa.sharedSizeBytes;      // side <= 83 on an H100 (227 KB)
+    std::vector<int32_t> nn_rows, soc_warp, soc_cta, soc_dim, psd_smem, psd_glob;
+    std::vector<int64_t> soc_moff, soc_srow, psd_moff, psd_loff, psd_woff;
+    int64_t moff = 0, srow = 0, loff = 0, wtot = 0, max_smem_side = 0;
+    int32_t socid = 0, psdid = 0;
+    for (size_t i = 0; i < h->h_ctype.size(); ++i) {
+        const int t = h->h_ctype[i];
+        const int64_t d = h->h_cdim[i];
+        if (t == 1) {
+            for (int64_t k = 0; k < d; ++k) nn_rows.push_back((int32_t)(moff + k));
+        } else if (t == 2) {
+            (d >= SOC_CTA_MIN_DIM ? soc_cta : soc_warp).push_back(socid++);
+            soc_dim.push_back((int32_t)d); soc_moff.push_back(moff); soc_srow.push_back(srow);
+            srow += d;
+        } else if (t == 3) {
+            if (32 * d * d <= dyn_cap) { psd_smem.push_back(psdid); max_smem_side = std::max(max_smem_side, d); }
+            else { psd_glob.push_back(psdid); psd_woff.push_back(wtot); wtot += 4 * d * d; }
+            psd_moff.push_back(moff); psd_loff.push_back(loff);
+            loff += d; psdid++;
+        }
+        moff += t == 3 ? d * (d + 1) / 2 : d;
+    }
+    cudaStream_t s = h->stream;
+    h->nnn = (int64_t)nn_rows.size();
+    h->nsoc_warp = (int32_t)soc_warp.size(); h->nsoc_cta = (int32_t)soc_cta.size();
+    h->npsd_smem = (int32_t)psd_smem.size(); h->npsd_glob = (int32_t)psd_glob.size();
+    h->psd_ltotal = loff;
+    soc_warp.insert(soc_warp.end(), soc_cta.begin(), soc_cta.end());
+    psd_smem.insert(psd_smem.end(), psd_glob.begin(), psd_glob.end());
+    CUDA_OK(h->d_nn_rows.upload(nn_rows, s));
+    CUDA_OK(h->d_soc_list.upload(soc_warp, s)); CUDA_OK(h->d_soc_dim.upload(soc_dim, s));
+    CUDA_OK(h->d_soc_moff.upload(soc_moff, s)); CUDA_OK(h->d_soc_srow.upload(soc_srow, s));
+    CUDA_OK(h->d_psd_list.upload(psd_smem, s)); CUDA_OK(h->d_psd_moff.upload(psd_moff, s));
+    CUDA_OK(h->d_psd_loff.upload(psd_loff, s)); CUDA_OK(h->d_psd_woff.upload(psd_woff, s));
+    const int64_t m1 = std::max<int64_t>(1, h->m);
+    CUDA_OK(h->d_lam.alloc(m1)); CUDA_OK(h->d_ss.alloc(m1)); CUDA_OK(h->d_sz.alloc(m1));
+    CUDA_OK(h->d_psd_Rinv.alloc(std::max<int64_t>(1, h->psd_rtotal)));
+    CUDA_OK(h->d_psd_lam.alloc(std::max<int64_t>(1, loff)));
+    CUDA_OK(h->d_psd_ws.alloc(std::max<int64_t>(1, wtot), /*fill=*/false));
+    CUDA_OK(h->d_scale_flags.alloc(2));
+    h->psd_smem_bytes = (size_t)(32 * max_smem_side * max_smem_side);     // four n x n FP64 matrices
+    if (max_smem_side)
+        CUDA_OK(cudaFuncSetAttribute(k_scale_psd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)h->psd_smem_bytes));
+    for (cudaEvent_t& e : h->ev_scale) if (!e) CUDA_OK(cudaEventCreate(&e));
+    CUDA_OK(cudaStreamSynchronize(s));
+    h->scale_ready = true;
+    return 0;
+}
+
+int32_t cb200_update_scaling(cb200_handle* h, const double* s, const double* z, int32_t* ok_scale) {
+    if (!h->maps_set) { set_error("cb200_update_scaling: cb200_set_maps not called"); return -2; }
+    for (int32_t t : h->h_ctype)
+        if (t >= 4) {
+            set_error("cb200_update_scaling: exponential, power and generalised power cones keep their host scaling");
+            return -2;
+        }
+    if ((!s || !z) && h->m) { set_error("cb200_update_scaling: s and z are required"); return -2; }
+    try {
+        CUDA_OK(cudaSetDevice(h->st.device));
+        int rc = prepare_scaling(h);
+        if (rc) return rc;
+        cudaStream_t st = h->stream;
+        const int64_t m = h->m;
+        // host pointers normally, device pointers in resident mode (read in place)
+        const double* ds = s;
+        const double* dz = z;
+        if (!h->resident && m) {
+            CUDA_OK(cudaMemcpyAsync(h->d_ss.p, s, m * sizeof(double), cudaMemcpyHostToDevice, st));
+            CUDA_OK(cudaMemcpyAsync(h->d_sz.p, z, m * sizeof(double), cudaMemcpyHostToDevice, st));
+            ds = h->d_ss.p; dz = h->d_sz.p;
+        }
+        CUDA_OK(cudaEventRecord(h->ev_scale[0], st));
+        CUDA_OK(cudaMemsetAsync(h->d_scale_flags.p, 0, 2 * sizeof(int), st));
+        int* fl = h->d_scale_flags.p;
+        if (h->nnn) {
+            k_scale_nn<<<nblk(h->nnn, SCALE_THREADS), SCALE_THREADS, 0, st>>>(h->nnn, h->d_nn_rows.p, ds, dz, h->d_w.p,
+                                                                             h->d_lam.p);
+            LAUNCH(h);
+        }
+        if (h->nsoc_warp) {
+            k_scale_soc<32><<<nblk(h->nsoc_warp, SCALE_THREADS / 32), SCALE_THREADS, 0, st>>>(
+                h->nsoc_warp, h->d_soc_list.p, h->d_soc_moff.p, h->d_soc_dim.p, h->d_soc_srow.p, ds, dz, h->d_w.p,
+                h->d_lam.p, h->d_eta.p, h->d_socd.p, h->d_socu.p, h->d_socv.p, fl);
+            LAUNCH(h);
+        }
+        if (h->nsoc_cta) {
+            k_scale_soc<SCALE_THREADS><<<h->nsoc_cta, SCALE_THREADS, 0, st>>>(
+                h->nsoc_cta, h->d_soc_list.p + h->nsoc_warp, h->d_soc_moff.p, h->d_soc_dim.p, h->d_soc_srow.p, ds, dz,
+                h->d_w.p, h->d_lam.p, h->d_eta.p, h->d_socd.p, h->d_socu.p, h->d_socv.p, fl);
+            LAUNCH(h);
+        }
+        constexpr int kMaxSweeps = 30;
+        if (h->npsd_smem) {
+            k_scale_psd<true><<<h->npsd_smem, SCALE_THREADS, h->psd_smem_bytes, st>>>(
+                h->d_psd_list.p, h->d_psd_side.p, h->d_psd_moff.p, h->d_psd_roff.p, h->d_psd_loff.p, nullptr, ds, dz,
+                nullptr, h->d_psd_R.p, h->d_psd_Rinv.p, h->d_psd_lam.p, fl, kMaxSweeps);
+            LAUNCH(h);
+        }
+        if (h->npsd_glob) {
+            k_scale_psd<false><<<h->npsd_glob, SCALE_THREADS, 0, st>>>(
+                h->d_psd_list.p + h->npsd_smem, h->d_psd_side.p, h->d_psd_moff.p, h->d_psd_roff.p, h->d_psd_loff.p,
+                h->d_psd_woff.p, ds, dz, h->d_psd_ws.p, h->d_psd_R.p, h->d_psd_Rinv.p, h->d_psd_lam.p, fl, kMaxSweeps);
+            LAUNCH(h);
+        }
+        CUDA_OK(cudaEventRecord(h->ev_scale[1], st));
+        CUDA_OK(cudaGetLastError());
+        int flags[2] = {0, 0};
+        CUDA_OK(cudaMemcpyAsync(flags, fl, sizeof(flags), cudaMemcpyDeviceToHost, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+        float ms = 0.f;
+        CUDA_OK(cudaEventElapsedTime(&ms, h->ev_scale[0], h->ev_scale[1]));
+        h->scale_ms += ms;
+        h->last_sweeps = flags[1];
+        if (ok_scale) *ok_scale = flags[0] ? 0 : 1;
+        return 0;
+    } catch (const std::exception& e) { set_error(e.what()); return -1; }
+}
+
+int32_t cb200_get_scaling(cb200_handle* h, double* w, double* lam, double* eta, double* d, double* u, double* v,
+                          double* R, double* Rinv, double* psd_lam) {
+    if (!h->maps_set) { set_error("cb200_get_scaling: cb200_set_maps not called"); return -2; }
+    try {
+        CUDA_OK(cudaSetDevice(h->st.device));
+        int rc = prepare_scaling(h);
+        if (rc) return rc;
+        cudaStream_t st = h->stream;
+        auto get = [&](double* dst, const double* src, int64_t len) -> cudaError_t {
+            if (!dst || len <= 0) return cudaSuccess;
+            return cudaMemcpyAsync(dst, src, len * sizeof(double), cudaMemcpyDeviceToHost, st);
+        };
+        CUDA_OK(get(w, h->d_w.p, h->m)); CUDA_OK(get(lam, h->d_lam.p, h->m));
+        CUDA_OK(get(eta, h->d_eta.p, h->nsoc)); CUDA_OK(get(d, h->d_socd.p, h->nsoc));
+        CUDA_OK(get(u, h->d_socu.p, h->nsocrows)); CUDA_OK(get(v, h->d_socv.p, h->nsocrows));
+        CUDA_OK(get(R, h->d_psd_R.p, h->psd_rtotal)); CUDA_OK(get(Rinv, h->d_psd_Rinv.p, h->psd_rtotal));
+        CUDA_OK(get(psd_lam, h->d_psd_lam.p, h->psd_ltotal));
+        CUDA_OK(cudaStreamSynchronize(st));
+        return 0;
+    } catch (const std::exception& e) { set_error(e.what()); return -1; }
 }
 
 int32_t cb200_setrhs(cb200_handle* h, const double* rhsx, const double* rhsz) {
@@ -1978,9 +2145,9 @@ int32_t cb200_download(cb200_handle* h, int32_t what, double* out, int64_t len) 
 }
 
 int32_t cb200_get_timers(cb200_handle* h, double* out, int32_t len) {
-    double v[11] = {h->tm.ms[0], h->tm.ms[1], h->tm.ms[2], h->tm.ms[3], h->tm.nfactor, h->tm.nsolve, h->tm.nlaunch,
-                    h->tm.ms[4], h->tm.ms[5], h->tm.ms[6], h->tm.ms[7]};
-    for (int i = 0; i < len && i < 11; ++i) out[i] = v[i];
+    double v[12] = {h->tm.ms[0], h->tm.ms[1], h->tm.ms[2], h->tm.ms[3], h->tm.nfactor, h->tm.nsolve, h->tm.nlaunch,
+                    h->tm.ms[4], h->tm.ms[5], h->tm.ms[6], h->tm.ms[7], h->scale_ms};
+    for (int i = 0; i < len && i < 12; ++i) out[i] = v[i];
     return 0;
 }
 int32_t cb200_nccl_unique_id(char out[128]) {
@@ -2071,14 +2238,15 @@ int32_t cb200_get_stats(const cb200_handle* h, double* out, int32_t len) {
         }
         if (nf * ns >= 65536 && ns > 32) big_bytes += 8.0 * nf * ns;
     }
-    double v[23] = {S.flops, schur, panel_large - schur, (double)S.nnzL, (double)S.nlevels, (double)S.nsuper,
+    double v[26] = {S.flops, schur, panel_large - schur, (double)S.nnzL, (double)S.nlevels, (double)S.nsuper,
                     nlarge, big_bytes, (double)S.upd_total * 8.0, (double)S.panel_off.back() * 8.0,
                     (double)S.ordering_used, my_flops, h->use_tma ? 1.0 : 0.0, (double)h->tma_kmajor,
                     (double)((h->g_factor[0].exec != nullptr) + (h->g_factor[1].exec != nullptr)),
                     h->g_solve.exec ? 1.0 : 0.0, (double)h->nsub,
                     (double)h->n_schur_tiles, (double)h->n_schur_rects, (double)h->n_asm_tiles, (double)h->n_asm_rects,
-                    h->n_multi_sweeps, h->n_percol};
-    for (int i = 0; i < len && i < 23; ++i) out[i] = v[i];
+                    h->n_multi_sweeps, h->n_percol,
+                    (double)h->npsd_smem, (double)h->npsd_glob, h->last_sweeps};
+    for (int i = 0; i < len && i < 26; ++i) out[i] = v[i];
     return 0;
 }
 
@@ -2087,6 +2255,7 @@ int32_t cb200_set_resident(cb200_handle* h, int32_t resident) { h->resident = re
 int32_t cb200_reset_timers(cb200_handle* h) {
     for (double& x : h->tm.ms) x = 0;
     h->tm.nfactor = h->tm.nsolve = h->tm.nlaunch = 0;
+    h->scale_ms = 0;
     return 0;
 }
 

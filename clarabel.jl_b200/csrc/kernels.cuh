@@ -14,6 +14,7 @@
 //                                         kernels_multi.cuh
 //   G8  symmetric SpMV residual + norm    k_residual, k_residual_long
 //   G9  multi-GPU helpers                 k_zero_panels, k_mask_vec  (collectives: api_cuda.cu)
+//   G10 NT scaling of the symmetric cones k_scale_nn, k_scale_soc, k_scale_psd: kernels_scaling.cuh
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -102,11 +102,11 @@ class B200DirectLDLSolver:
         return out
 
     def timers(self):
-        out = np.zeros(11)
-        self._L.cb200_get_timers(self._h, _p(out), 11)
+        out = np.zeros(12)
+        self._L.cb200_get_timers(self._h, _p(out), 12)
         return dict(cone_ms=out[0], factor_ms=out[1], solve_ms=out[2], spmv_ms=out[3],
                     nfactor=int(out[4]), nsolve=int(out[5]), nlaunch=int(out[6]),
-                    schur_ms=out[7], panel_ms=out[8], small_ms=out[9], asm_ms=out[10])
+                    schur_ms=out[7], panel_ms=out[8], small_ms=out[9], asm_ms=out[10], scale_ms=out[11])
 
     def set_detail(self, level):
         """0 off, 1 (or True) factorisation groups, 2 every kernel class (see fine_timers)."""
@@ -120,12 +120,12 @@ class B200DirectLDLSolver:
         return {self._L.cb200_fine_timer_name(i).decode(): float(out[i]) for i in range(n)}
 
     def stats(self):
-        out = np.zeros(23)
-        self._L.cb200_get_stats(self._h, _p(out), 23)
+        out = np.zeros(26)
+        self._L.cb200_get_stats(self._h, _p(out), 26)
         keys = ["flops", "schur_flops", "panel_flops", "nnzL", "nlevels", "nsuper", "nlarge",
                 "big_solve_bytes", "upd_bytes", "panel_bytes", "ordering_used", "rank_flops", "use_tma", "tma_kmajor",
                 "factor_graphs", "solve_graph", "subtrees", "schur_tiles", "schur_rects", "asm_tiles", "asm_rects",
-                "multi_sweeps", "multi_percol"]
+                "multi_sweeps", "multi_percol", "psd_scale_smem", "psd_scale_global", "jacobi_sweeps"]
         return dict(zip(keys, out.tolist()))
 
     def reset_timers(self):
@@ -225,7 +225,10 @@ class B200KKTSolver:
             if not hasattr(self, "_ns_idx"):
                 self._ns_idx = nonsym_update_index(self.map, cones)
             self.ldl.update_values(self._ns_idx, nonsym_update_values(self.map, cones))
-        if self.ldl.resident:      # host arrays are not read in resident mode: refactor the state in HBM
+        if self.ldl.resident or self._state_on_device:
+            # resident mode reads no host array, and after update_scaling the device already holds the state:
+            # refactor from the state in HBM
+            self._state_on_device = False
             return _lib.check(self.ldl._L.cb200_update_cones(self.ldl._h, *([None] * 6)), "cb200_update_cones")
         st = cones.export_state()
         arrs = [_c64(st[k]) for k in ("w", "soc_eta", "soc_d", "soc_u", "soc_v", "psd_R")]
@@ -233,6 +236,57 @@ class B200KKTSolver:
                           "cb200_update_cones")
 
     STATE_KEYS = ("w", "soc_eta", "soc_d", "soc_u", "soc_v", "psd_R")
+    _state_on_device = False
+
+    def update_scaling(self, s, z, cones):
+        """update_scaling! of the symmetric cones on the device (cb200_update_scaling).  The state goes back into
+        the CompositeCone fields the host cone operations read (w, lam, soc_eta/d/u/v, psd_groups R / Rinv / lam),
+        and the next update(cones) refactors from the device copy instead of uploading it.  Returns ok_scale:
+        False exactly where cones.update_scaling returns False.  In resident mode s and z are device addresses
+        (int) and nothing is downloaded."""
+        L, h = self.ldl._L, self.ldl._h
+        ok = C.c_int32(0)
+        if self.ldl.resident:
+            _lib.check(L.cb200_update_scaling(h, C.c_void_p(s), C.c_void_p(z), C.byref(ok)), "cb200_update_scaling")
+            return bool(ok.value)
+        sv, zv = _c64(s), _c64(z)
+        _lib.check(L.cb200_update_scaling(h, _p(sv), _p(zv), C.byref(ok)), "cb200_update_scaling")
+        if not ok.value:
+            return False
+        self.download_scaling(cones)
+        self._state_on_device = True
+        return True
+
+    def download_scaling(self, cones):
+        """Copy the device scaling state into the CompositeCone fields (cb200_get_scaling)."""
+        if not hasattr(self, "_psd_slots"):
+            # (group, position in group, side) of every PSD cone in cone order: the device keeps them in cone order
+            slot = {}
+            for gi, g in enumerate(cones.psd_groups):
+                for j, ci in enumerate(g["cones"]):
+                    slot[int(ci)] = (gi, j, g["n"])
+            self._psd_slots = [slot[i] for i in sorted(slot)]
+            self._psd_rtotal = sum(n * n for _, _, n in self._psd_slots)
+            self._psd_ltotal = sum(n for _, _, n in self._psd_slots)
+            # rows of w / λ that update_scaling writes (NN and SOC); the others keep their host values
+            self._wl_rows = np.zeros(cones.numel, dtype=bool)
+            self._wl_rows[cones.nn_idx] = True; self._wl_rows[cones.soc_idx] = True
+        m = cones.numel
+        direct = bool(self._wl_rows.all()) and cones.w.flags.c_contiguous and cones.lam.flags.c_contiguous
+        w, lam = (cones.w, cones.lam) if direct else (np.empty(m), np.empty(m))
+        R, Ri, pl = np.empty(self._psd_rtotal), np.empty(self._psd_rtotal), np.empty(self._psd_ltotal)
+        _lib.check(self.ldl._L.cb200_get_scaling(self.ldl._h, *[_p(a) for a in (w, lam, cones.soc_eta, cones.soc_d,
+                                                                              cones.soc_u, cones.soc_v, R, Ri, pl)]),
+                   "cb200_get_scaling")
+        if not direct:
+            np.copyto(cones.w, w, where=self._wl_rows); np.copyto(cones.lam, lam, where=self._wl_rows)
+        ro = lo = 0
+        for gi, j, n in self._psd_slots:
+            g = cones.psd_groups[gi]
+            g["R"][j] = R[ro:ro + n * n].reshape((n, n), order="F")
+            g["Rinv"][j] = Ri[ro:ro + n * n].reshape((n, n), order="F")
+            g["lam"][j] = pl[lo:lo + n]
+            ro += n * n; lo += n
 
     def update_staged(self, dev_ptrs):
         """Resident mode: kktsolver_update! from a cone state the caller has staged in HBM.

@@ -18,7 +18,7 @@ EXPORTED = [
     "cb200_order_amd", "cb200_order_nd",
     "cb200_create", "cb200_destroy", "cb200_update_values", "cb200_scale_values",
     "cb200_refactor", "cb200_solve", "cb200_solve_multi", "cb200_info",
-    "cb200_set_maps", "cb200_update_cones", "cb200_setrhs", "cb200_solve_ir", "cb200_solve_ir_multi", "cb200_update_P", "cb200_update_A",
+    "cb200_set_maps", "cb200_update_cones", "cb200_update_scaling", "cb200_get_scaling", "cb200_setrhs", "cb200_solve_ir", "cb200_solve_ir_multi", "cb200_update_P", "cb200_update_A",
     "cb200_download", "cb200_get_timers", "cb200_reset_timers", "cb200_last_error",
     "cb200_get_stream", "cb200_set_resident",
     "cb200_symbolic_partition", "cb200_nccl_unique_id", "cb200_dist_init",
@@ -74,6 +74,8 @@ def lib():
         L.cb200_set_maps.argtypes = [P, I64, I64, I64, P, I64, P, I64, P, I64, P, I64, P, P, P, P, P]
         L.cb200_set_maps.restype = I32
         L.cb200_update_cones.argtypes = [P] * 7; L.cb200_update_cones.restype = I32
+        L.cb200_update_scaling.argtypes = [P] * 4; L.cb200_update_scaling.restype = I32
+        L.cb200_get_scaling.argtypes = [P] * 10; L.cb200_get_scaling.restype = I32
         L.cb200_solve_ir.argtypes = [P] * 6; L.cb200_solve_ir.restype = I32
         L.cb200_solve_ir_multi.argtypes = [P, I32] + [P] * 6; L.cb200_solve_ir_multi.restype = I32
         L.cb200_setrhs.argtypes = [P, P, P]; L.cb200_setrhs.restype = I32

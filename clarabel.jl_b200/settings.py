@@ -67,3 +67,6 @@ class Settings:
 
     # B200 backend knobs (no reference counterpart)
     b200_devices: tuple = field(default_factory=tuple)   # () = current device only
+    # compute the NT scaling of symmetric cones on the device (cb200_update_scaling) instead of on the host;
+    # used with direct_solve_method="b200" when every cone is Zero / NN / SOC / PSD
+    b200_device_cone_scaling: bool = False

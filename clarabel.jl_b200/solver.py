@@ -425,6 +425,8 @@ class Solver:
         self.iter_log = []
         sym = cones.is_symmetric
         scaling = PRIMAL_DUAL if cones.allows_primal_dual_scaling else DUAL
+        # NT scaling of the symmetric cones on the device (the state stays there for the next kkt update)
+        device_scaling = st.b200_device_cone_scaling and st.direct_solve_method == "b200" and sym
         while True:
             r.update(v, data)
             mu = (r.dot_sz + v.tau * v.kappa) / (cones.degree + 1)
@@ -446,7 +448,10 @@ class Solver:
                         continue
                 break
             t = time.perf_counter()
-            ok_scale = cones.update_scaling(v.s, v.z, mu, scaling)
+            if device_scaling:
+                ok_scale = self.kktsystem.kktsolver.update_scaling(v.s, v.z, cones)
+            else:
+                ok_scale = cones.update_scaling(v.s, v.z, mu, scaling)
             tm["scale cones"] += time.perf_counter() - t
             if not ok_scale:
                 info.status = NUMERICAL_ERROR

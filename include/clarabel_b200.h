@@ -134,10 +134,26 @@ int32_t cb200_set_maps(cb200_handle* h, int64_t n, int64_t m, int64_t p,
 /* kktsolver_update!(ks, cones)::Bool — kktsolver_directldl.jl:197-294 (get_Hs!, sign flip,
  * sparse-cone scatter, static regularisation, refactor).  Cone scaling state as produced by
  * update_scaling! on the host: w over all m rows (NN: w, SOC: w), per-SOC eta and d, SOC u/v
- * over all SOC rows, PSD R matrices (column-major n*n each, cone order). */
+ * over all SOC rows, PSD R matrices (column-major n*n each, cone order).  A NULL argument keeps
+ * that part of the state on the device (the previous upload, or what cb200_update_scaling
+ * computed), in both modes. */
 int32_t cb200_update_cones(cb200_handle* h, const double* w, const double* soc_eta,
                            const double* soc_d, const double* soc_u, const double* soc_v,
                            const double* psd_R);
+/* update_scaling!(cones, s, z, μ, strategy) for symmetric cones — coneops_nncone.jl:77-89,
+ * coneops_socone.jl:75-154, coneops_psdtrianglecone.jl:78-143 — on the device.  s and z have length m (host
+ * pointers; device pointers under cb200_set_resident).  Writes the state cb200_update_cones reads (w, eta, d, u, v,
+ * PSD R), so that cb200_update_cones(h, NULL, ..., NULL) refactors from it, plus λ (NN/SOC rows), PSD Rinv and PSD
+ * λ for the host cone operations (cb200_get_scaling).  *ok_scale = 0 where the host returns false: a SOC residual
+ * of z, s or w not > 0 (NaN included), a Cholesky pivot of S or Z not > 0, or a Jacobi SVD of L2'L1 that has not
+ * converged in 30 sweeps; NN cones are not checked.  PSD λ is not sorted (R, Rinv and λ agree with each other).
+ * Returns -2 if the cone table has exponential, power or generalised power cones (types 4-6): they keep their host
+ * scaling.  In multi-GPU mode every rank computes the whole state from its own (replicated) s and z. */
+int32_t cb200_update_scaling(cb200_handle* h, const double* s, const double* z, int32_t* ok_scale);
+/* Download the scaling state into host arrays; NULL skips an array.  Lengths: w, lam m; eta, d #SOC; u, v the SOC
+ * rows; R, Rinv the sum of n*n over the PSD cones (column-major each, cone order); psd_lam the sum of n. */
+int32_t cb200_get_scaling(cb200_handle* h, double* w, double* lam, double* eta, double* d, double* u, double* v,
+                          double* R, double* Rinv, double* psd_lam);
 /* kktsolver_setrhs!(ks, rhsx, rhsz) — kktsolver_directldl.jl:313-327: b = [rhsx; rhsz; 0_p].  The
  * right-hand side is copied to the device here (the caller may reuse its buffers on return);
  * a following cb200_solve_ir with rhsx == rhsz == NULL solves for it. */
@@ -181,7 +197,8 @@ int32_t cb200_download(cb200_handle* h, int32_t what, double* out, int64_t len);
  * 1 factor, 2 triangular solves, 3 spmv/residual ; counters: 4 #factor, 5 #solve sweeps (a multi-RHS sweep of
  * up to 4 columns counts once), 6 #kernel launches ;
  * with cb200_set_detail(h,1) also per kernel class inside the factorisation: 7 k_schur_large,
- * 8 pivot-block phase (k_diag64 + k_rows64), 9 small fronts (k_factor_small), 10 assembly */
+ * 8 pivot-block phase (k_diag64 + k_rows64), 9 small fronts (k_factor_small), 10 assembly ;
+ * 11 device time of cb200_update_scaling (its kernels, always recorded) */
 int32_t cb200_get_timers(cb200_handle* h, double* out, int32_t len);
 int32_t cb200_reset_timers(cb200_handle* h);
 /* event timing inside the phases (disables CUDA-graph replay while on): level 0 off, 1 the four
@@ -199,7 +216,9 @@ const char* cb200_fine_timer_name(int32_t i);
  * 14 factorisation graphs instantiated (0-2), 15 solve-sweep graph instantiated, 16 bottom subtrees
  * solved by k_fwd_subtree / k_bwd_subtree, 17 Schur tiles and 18 their child rectangles, 19 assembly
  * tiles and 20 their child rectangles (all large batches, cb200_symbolic_tile_lists), 21 multi-RHS sweeps run
- * batched, 22 columns of the multi-RHS calls solved one by one through the single-RHS path */
+ * batched, 22 columns of the multi-RHS calls solved one by one through the single-RHS path, 23 PSD cones
+ * scaled in shared memory and 24 in a global workspace by cb200_update_scaling, 25 Jacobi sweeps of its last call
+ * (maximum over the PSD cones) */
 int32_t cb200_get_stats(const cb200_handle* h, double* out, int32_t len);
 /* ---------------------------------------------------------------- multi-GPU (one process per GPU)
  * Every rank creates the same handle on its own device (replicated symbolic analysis), then

@@ -70,4 +70,20 @@ function linear_solver_info(s::B200DirectLDLSolver)
     ccall((:cb200_info, LIB), Int32, (Ptr{Cvoid}, Ref{Int64}, Ref{Int64}, Ref{Int32}), s.handle, nnzA, nnzL, ng)
     LinearSolverInfo(:b200, ng[], true, nnzA[], nnzL[])
 end
+
+# update_scaling! of the symmetric cones on the device (INTEGRATION.md, "Cone scaling on the device").  `h` is a
+# handle after cb200_set_maps; s, z have length m.  Returns ok_scale (false where update_scaling! returns false);
+# afterwards cb200_update_cones(h, C_NULL, ..., C_NULL) refactors from the device state.
+function b200_update_scaling!(h::Ptr{Cvoid}, s::Vector{Float64}, z::Vector{Float64})
+    ok = Ref{Int32}(0)
+    rc = ccall((:cb200_update_scaling, LIB), Int32, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Ref{Int32}), h, s, z, ok)
+    rc < 0 && error(unsafe_string(ccall((:cb200_last_error, LIB), Cstring, ())))
+    return ok[] != 0
+end
+# The state for the host cone operations; pass C_NULL for what is not needed.  w, lam: m; eta, d: #SOC; u, v: the
+# SOC rows; R, Rinv: sum of n^2 over the PSD cones (column-major, cone order); psd_lam: sum of n.
+b200_get_scaling!(h::Ptr{Cvoid}, w, lam, eta, d, u, v, R, Rinv, psd_lam) =
+    _chk(ccall((:cb200_get_scaling, LIB), Int32,
+               (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
+                Ptr{Float64}, Ptr{Float64}, Ptr{Float64}), h, w, lam, eta, d, u, v, R, Rinv, psd_lam))
 end # module
