@@ -1663,8 +1663,6 @@ int32_t cb200_set_maps(cb200_handle* h, int64_t n, int64_t m, int64_t p,
         CUDA_OK(h->d_eta.alloc(std::max<int64_t>(1, h->nsoc))); CUDA_OK(h->d_socd.alloc(std::max<int64_t>(1, h->nsoc)));
         CUDA_OK(h->d_socu.alloc(std::max<int64_t>(1, socrow))); CUDA_OK(h->d_socv.alloc(std::max<int64_t>(1, socrow)));
         CUDA_OK(h->d_rx.alloc(std::max<int64_t>(1, n))); CUDA_OK(h->d_rz.alloc(std::max<int64_t>(1, m)));
-        if (h->psd_maxn) CUDA_OK(cudaFuncSetAttribute(k_psd_skron, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                      std::max(48 * 1024, h->psd_maxn * h->psd_maxn * 8)));
         h->h_ctype.assign(cone_type, cone_type + ncones); h->h_cdim.assign(cone_dim, cone_dim + ncones);
         h->scale_ready = false;
         CUDA_OK(cudaStreamSynchronize(s));
@@ -1711,8 +1709,7 @@ int32_t cb200_update_cones(cb200_handle* h, const double* w, const double* soc_e
     if (h->npsd) {
         k_psd_rrt<<<h->npsd, 256, 0, st>>>(h->d_psd_side.p, h->d_psd_roff.p, h->d_psd_R.p, h->d_psd_A.p);
         const int ne = h->psd_maxn * (h->psd_maxn + 1) / 2;
-        k_psd_skron<<<dim3(std::max(1, std::min(64, nblk(ne, 8))), h->npsd), 256,
-                      (size_t)h->psd_maxn * h->psd_maxn * sizeof(double), st>>>(
+        k_psd_skron<<<dim3(std::max(1, std::min(64, nblk(ne, 8))), h->npsd), 256, 0, st>>>(
             h->d_psd_side.p, h->d_psd_roff.p, h->d_psd_hoff.p, h->d_psd_A.p, h->d_mapHs.p, h->d_nz.p);
         h->tm.nlaunch += 2;
     }
@@ -2129,6 +2126,7 @@ int32_t cb200_download(cb200_handle* h, int32_t what, double* out, int64_t len) 
                   CUDA_OK(cudaStreamSynchronize(st)); out[0] = (double)v; return 0; }
         case 6: src = h->d_x.p; n = h->N; break;       // full solution [x; z; expansion variables] of the last solve
         case 8: src = h->d_msol.p; n = h->N * h->msol_cols; break;   // the same, N x nrhs, of the last cb200_solve_ir_multi
+        case 9: src = h->d_e.p; n = h->N; break;       // residual b - K x last computed by cb200_solve_ir
         case 7: { if (len != 64) { set_error("download: length"); return -2; }     // ORIGINAL indices of the first 64 regularised pivots
                   int32_t v[64]; unsigned int cnt = 0;
                   CUDA_OK(cudaMemcpyAsync(v, h->d_reglog.p, sizeof(v), cudaMemcpyDeviceToHost, st));

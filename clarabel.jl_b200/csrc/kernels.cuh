@@ -2254,17 +2254,17 @@ k_psd_rrt(const int32_t* __restrict__ side, const int64_t* __restrict__ roff,
 }
 // k_psd_skron: grid (column tiles, cones).  Column q=(k,l), row p=(i,j) of triu(A (x)_s A)
 // (skron!, coneops_psdtrianglecone.jl:502-540); writes -value through the Hs map.
+// A is read through the read-only cache rather than staged in shared memory: it is 8 n^2 bytes
+// per cone and stays in L1 / L2, and staging would cap the side at what one block's shared
+// memory holds (n = 170 on an H100).
 __global__ void __launch_bounds__(256)
 k_psd_skron(const int32_t* __restrict__ side, const int64_t* __restrict__ roff,
             const int64_t* __restrict__ hoff, const double* __restrict__ A,
             const int64_t* __restrict__ map, double* __restrict__ nz) {
-    extern __shared__ double sA[];
     const int c = blockIdx.y;
     const int n = side[c];
     const int ne = n * (n + 1) / 2;
     const double* Ac = A + roff[c];
-    for (int e = threadIdx.x; e < n * n; e += blockDim.x) sA[e] = Ac[e];
-    __syncthreads();
     const int64_t* mp = map + hoff[c];
     const double s2 = sqrt(2.0);
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -2283,11 +2283,11 @@ k_psd_skron(const int32_t* __restrict__ side, const int64_t* __restrict__ roff,
             while (j * (j + 1) / 2 > p) --j;
             const int i = p - j * (j + 1) / 2;
             const bool ij = (i == j);
-            const double Ajl = sA[j + l * n], Ajk = sA[j + k * n];
+            const double Ajl = __ldg(Ac + j + l * n), Ajk = __ldg(Ac + j + k * n);
             double v;
-            if (!ij && !kl) v = sA[i + k * n] * Ajl + sA[i + l * n] * Ajk;
+            if (!ij && !kl) v = __ldg(Ac + i + k * n) * Ajl + __ldg(Ac + i + l * n) * Ajk;
             else if (ij && !kl) v = s2 * Ajl * Ajk;
-            else if (!ij && kl) v = s2 * sA[i + l * n] * Ajk;
+            else if (!ij && kl) v = s2 * __ldg(Ac + i + l * n) * Ajk;
             else v = Ajl * Ajl;
             nz[mp[cbase + p]] = -v;
         }

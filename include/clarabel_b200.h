@@ -191,7 +191,11 @@ int32_t cb200_update_A(cb200_handle* h, const double* values, int64_t len);
  *       3 perm (as doubles), 4 last static regulariser (len 1), 5 regularised-pivot count (len 1),
  *       6 full solution [x; z; expansion variables] of the last solve (len N),
  *       7 original indices of the first 64 dynamically regularised pivots of the last factorisation (len 64, -1 = none),
- *       8 full solutions of the last cb200_solve_ir_multi, N x nrhs column-major (len N * nrhs) */
+ *       8 full solutions of the last cb200_solve_ir_multi, N x nrhs column-major (len N * nrhs),
+ *       9 residual e = b - K x (unregularised K) last computed by cb200_solve_ir (len N): x is the last
+ *         iterate refinement tried, which is the returned solution unless the final round was rejected
+ *         (with iterative_refinement_max_iter = 0 it is the unrefined solve); not written when
+ *         refinement is disabled */
 int32_t cb200_download(cb200_handle* h, int32_t what, double* out, int64_t len);
 /* timers (ms, accumulated CUDA-event times on the handle's stream): 0 cone update + scatter,
  * 1 factor, 2 triangular solves, 3 spmv/residual ; counters: 4 #factor, 5 #solve sweeps (a multi-RHS sweep of

@@ -38,6 +38,70 @@ def kkt_fixture(cb, gen, seed=0):
     return KKT, mp, Ds, data, cones
 
 
+def cone_table_problem(cb, specs, n=8, seed=0, extra_A=None):
+    """(P, A, cones) for a designed cone table: P diagonal positive definite, A (m x n) with one entry
+    in every row plus a few random ones, so that K is quasidefinite whatever the cone state.
+    extra_A: optional dense m x n array added to A (dense rows / columns)."""
+    cones = cb.CompositeCone(specs)
+    m = cones.numel
+    rng = np.random.default_rng(seed)
+    P = sp.diags(1.0 + rng.random(n)).tocsc()
+    A = sp.csc_matrix((rng.standard_normal(m), (np.arange(m), rng.integers(0, n, m))), shape=(m, n))
+    A = A + sp.random(m, n, density=min(1.0, 2.0 / n), random_state=seed, data_rvs=rng.standard_normal)
+    if extra_A is not None:
+        A = A + sp.csc_matrix(extra_A)
+    A = A.tocsc(); A.sort_indices()
+    return P, A, cones
+
+
+def set_interior_scaling(cones, seed, spread=0.0):
+    """cones.update_scaling at a random interior point (s, z); NN / SOC / PSD scales spread over
+    10^(+-spread).  Nonsymmetric cones keep the unit initialisation point."""
+    m = cones.numel
+    rng = np.random.default_rng(seed)
+    z, s = np.zeros(m), np.zeros(m)
+    cones.unit_initialization(z, s)
+    sc = lambda k: 10.0 ** rng.uniform(-spread, spread, k)
+    ni = cones.nn_idx
+    s[ni] = sc(len(ni)) * (0.5 + rng.random(len(ni))); z[ni] = sc(len(ni)) * (0.5 + rng.random(len(ni)))
+    for v in (s, z):
+        for ci in cones.soc_cones:
+            a, b = int(cones.rng_cones[ci]), int(cones.rng_cones[ci + 1])
+            t = rng.standard_normal(b - a - 1)
+            v[a] = np.linalg.norm(t) * (1.0 + rng.random()) + 0.1
+            v[a + 1:b] = t
+            v[a:b] *= sc(1)
+        for g in cones.psd_groups:
+            k, nn = len(g["cones"]), g["n"]
+            M = rng.standard_normal((k, nn, nn))
+            S = (M @ np.swapaxes(M, 1, 2)) / nn + 0.2 * np.eye(nn)
+            S *= sc(k)[:, None, None]
+            v[g["idx"]] = cones._psd_svec(g, S)
+    assert cones.update_scaling(s, z, 1.0)
+    return s, z
+
+
+def set_synthetic_state(cones, seed, spread=8.0):
+    """A scaling state written field by field: NN w and SOC eta over 10^(+-spread), SOC w unit
+    hyperbolic (w0 = sqrt(1 + |w1|^2)) with |w1| over the same range, arbitrary d, u, v, PSD R with
+    entries over 10^(+-spread / 4)."""
+    rng = np.random.default_rng(seed)
+    sc = lambda k: 10.0 ** rng.uniform(-spread, spread, k)
+    cones.w[cones.nn_idx] = sc(len(cones.nn_idx))
+    for ci in cones.soc_cones:
+        a, b = int(cones.rng_cones[ci]), int(cones.rng_cones[ci + 1])
+        t = rng.standard_normal(b - a - 1) * sc(1)
+        cones.w[a + 1:b] = t
+        cones.w[a] = np.sqrt(1.0 + t @ t)
+    if cones.nsoc:
+        cones.soc_eta[:] = sc(cones.nsoc)
+        cones.soc_d[:] = rng.random(cones.nsoc)
+        cones.soc_u[:] = rng.standard_normal(len(cones.soc_u)) * sc(len(cones.soc_u))
+        cones.soc_v[:] = rng.standard_normal(len(cones.soc_v)) * sc(len(cones.soc_v))
+    for g in cones.psd_groups:
+        g["R"][:] = rng.standard_normal(g["R"].shape) * 10.0 ** rng.uniform(-spread / 4, spread / 4, g["R"].shape)
+
+
 def sym_full(K):
     return (K + sp.triu(K, 1).T).tocsc()
 
