@@ -191,6 +191,7 @@ struct cb200_handle {
     DevBuf<SolveDesc> d_sdesc;          // one packed descriptor per batch entry (same indexing as d_batches)
     DevBuf<int64_t> d_rows_ptr, d_panel_off, d_upd_off, d_woff, d_front_ptr, d_asm_base;
     DevBuf<int32_t> d_asm_colptr, d_asm_src, d_asm_child;
+    DevBuf<Symbolic::KidEntry> d_kids;
     // numeric
     DevBuf<double> d_L, d_U, d_W, d_D, d_Dinv, d_uvec, d_partial;
     DevBuf<BigItem> d_bigwork;
@@ -320,7 +321,7 @@ DevSym devsym(cb200_handle* h) {
     d.child_ptr = h->d_child_ptr.p; d.child_list = h->d_child_list.p;
     d.panel_off = h->d_panel_off.p; d.upd_off = h->d_upd_off.p; d.dsign = h->d_dsign_perm.p; d.ld = h->d_ld.p;
     d.front_ptr = h->d_front_ptr.p; d.asm_base = h->d_asm_base.p; d.asm_colptr = h->d_asm_colptr.p;
-    d.asm_src = h->d_asm_src.p; d.asm_child = h->d_asm_child.p;
+    d.asm_src = h->d_asm_src.p; d.asm_child = h->d_asm_child.p; d.kids = h->d_kids.p;
     d.active = h->dist ? h->d_active.p : nullptr;
     return d;
 }
@@ -336,14 +337,15 @@ struct FineScope {
     ~FineScope() { if (on) h->tm.end(h->stream); }
 };
 
-template <int T>
+// G threads per front, FPC fronts per CTA, each with an nf x nf front in shared memory
+template <int G, int FPC>
 int launch_small(cb200_handle* h, const Batch& b, int cls, RegParams rp, cudaStream_t st) {
     if (b.cnt == 0) return 0;
     FineScope fs(h, Timers::F_SMALL0 + cls);
-    const int sbuf = std::min(SB, b.maxns);
-    size_t sm = ((size_t)b.maxnf * b.maxnf + (size_t)sbuf * sbuf) * sizeof(double);
-    k_factor_small<T><<<b.cnt, T, sm, st>>>(devsym(h), h->d_batches.p + b.off, h->d_L.p,
-                                                   h->d_U.p, h->d_D.p, h->d_Dinv.p, rp, h->d_nreg.p);
+    const int fstride = b.maxnf * b.maxnf;
+    const size_t sm = (size_t)FPC * fstride * sizeof(double);
+    k_factor_small<G, FPC><<<nblk(b.cnt, FPC), G * FPC, sm, st>>>(devsym(h), h->d_batches.p + b.off, b.cnt, fstride,
+                                                                  h->d_L.p, h->d_U.p, h->d_D.p, h->d_Dinv.p, rp, h->d_nreg.p);
     LAUNCH(h);
     return 0;
 }
@@ -866,12 +868,12 @@ int factor_body(cb200_handle* h, bool static_reg) {
         cudaStream_t ss = ms ? h->side[0] : st;
         if (ms) h->fork(1);
         if (h->detail) h->tm.begin(Timers::SMALL, st);
-        launch_small<32>(h, P.small[0], 0, rp, ss);        // size classes kSmallNf[0..5]
-        launch_small<64>(h, P.small[1], 1, rp, ss);
-        launch_small<128>(h, P.small[2], 2, rp, ss);
-        launch_small<256>(h, P.small[3], 3, rp, ss);
-        launch_small<256>(h, P.small[4], 4, rp, ss);
-        launch_small<256>(h, P.small[5], 5, rp, ss);
+        launch_small<32, 8>(h, P.small[0], 0, rp, ss);     // size classes kSmallNf[0..5]: a warp per front
+        launch_small<64, 1>(h, P.small[1], 1, rp, ss);     // up to nf 16, a CTA per front above
+        launch_small<128, 1>(h, P.small[2], 2, rp, ss);
+        launch_small<256, 1>(h, P.small[3], 3, rp, ss);
+        launch_small<256, 1>(h, P.small[4], 4, rp, ss);
+        launch_small<256, 1>(h, P.small[5], 5, rp, ss);
         for (int c = 0; c < NPANEL; ++c) {
             const Batch& b = P.panel[c];
             if (!b.cnt) continue;
@@ -1403,7 +1405,7 @@ int32_t cb200_create(int64_t N, const int64_t* colptr, const int64_t* rowval, co
         CUDA_OK(h->d_ld.upload(S.panel_ld, s));
         CUDA_OK(h->d_front_ptr.upload(S.front_ptr, s)); CUDA_OK(h->d_asm_base.upload(S.asm_base, s));
         CUDA_OK(h->d_asm_colptr.upload(S.asm_colptr, s)); CUDA_OK(h->d_asm_src.upload(S.asm_src, s));
-        CUDA_OK(h->d_asm_child.upload(S.asm_child, s));
+        CUDA_OK(h->d_asm_child.upload(S.asm_child, s)); CUDA_OK(h->d_kids.upload(S.kids, s));
         // ---- level plans (+ workspace sized for them)
         { int rcp = build_plans(h); if (rcp) return rcp; }
         // ---- numeric storage
@@ -1422,12 +1424,8 @@ int32_t cb200_create(int64_t N, const int64_t* colptr, const int64_t* rowval, co
         CUDA_OK(cudaMemsetAsync(h->d_nreg.p, 0, sizeof(unsigned int), s));
         // opt in to large dynamic shared memory for the bigger small-front classes
         CUDA_OK(cudaFuncSetAttribute(k_factor_panel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-        CUDA_OK(cudaFuncSetAttribute(k_factor_small<256>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (152 * 152 + SB * SB) * (int)sizeof(double)));
-        CUDA_OK(cudaFuncSetAttribute(k_factor_small<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (64 * 64 + SB * SB) * (int)sizeof(double)));
-        CUDA_OK(cudaFuncSetAttribute(k_factor_small<64>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (32 * 32 + SB * SB) * (int)sizeof(double)));
+        CUDA_OK(cudaFuncSetAttribute(k_factor_small<256, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     152 * 152 * (int)sizeof(double)));
         CUDA_OK(cudaFuncSetAttribute(k_piv_rows, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (2 * PB * (PB + 1)) * (int)sizeof(double)));
         CUDA_OK(cudaFuncSetAttribute(k_ldl_update_tma<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tma_gemm_smem(128)));

@@ -132,6 +132,15 @@ int32_t cb200_symbolic_get(const cb200_symbolic* s, int32_t which, int64_t* out,
         case 8: return copy_out(S.a_map, out, len);     case 9: return copy_out(S.sn_level, out, len);
         case 10: return copy_out(S.child_ptr, out, len); case 11: return copy_out(S.child_list, out, len);
         case 12: return copy_out(S.panel_ld, out, len);
+        case 14: return copy_out(S.front_ptr, out, len); case 15: return copy_out(S.asm_base, out, len);
+        case 16: return copy_out(S.asm_colptr, out, len); case 17: return copy_out(S.asm_src, out, len);
+        case 18: return copy_out(S.asm_child, out, len);
+        case 13:
+            if ((int64_t)S.kids.size() * 3 != len) { cb200::set_error("cb200_symbolic_get: length mismatch"); return -2; }
+            for (size_t q = 0; q < S.kids.size(); ++q) {
+                out[3 * q] = S.kids[q].uoff; out[3 * q + 1] = S.kids[q].roff; out[3 * q + 2] = S.kids[q].nrc;
+            }
+            return 0;
     }
     cb200::set_error("cb200_symbolic_get: bad selector"); return -2;
 }

@@ -39,6 +39,7 @@ struct DevSym {                 // device copies of the Symbolic arrays
     const int32_t* asm_colptr;
     const int32_t* asm_src;
     const int32_t* asm_child;
+    const Symbolic::KidEntry* kids;   // per-front child lists of k_factor_small (symbolic.h)
     const int8_t*  active;      // multi-GPU: per-supernode mask of children whose contributions this rank
                                 // assembles into the replicated top fronts (nullptr = all)
 };
@@ -56,103 +57,128 @@ __device__ __forceinline__ void note_reg(const RegParams& rp, unsigned int* nreg
 // with no per-column dependency chain (chain length ns/SB instead of ns).
 constexpr int SB = 64;
 
-// Invert the unit-lower sb x sb block T (column-major, leading dimension ld) in place.
-// `buf` is scratch of SB*SB doubles in shared memory.  All threads of the CTA must call.
-__device__ __forceinline__ void invert_unit_lower_block(double* T, int ld, int sb, double* buf,
-                                                        int tid, int nthreads) {
-    for (int e = tid; e < sb * sb; e += nthreads) {
-        const int i = e % sb, j = e / sb;
-        buf[e] = (i > j) ? T[i + j * ld] : 0.0;
-    }
-    __syncthreads();
-    // column j of X = T^-1:  x_i = -sum_{k=j}^{i-1} T_ik x_k  (x_j = 1), one thread per column
-    for (int j = tid; j < sb; j += nthreads) {
-        double* X = T + j * ld;
-        for (int i = j + 1; i < sb; ++i) {
-            double acc = -buf[i + j * sb];                     // k = j term (x_j = 1)
-            for (int k = j + 1; k < i; ++k) acc -= buf[i + k * sb] * X[k];
-            X[i] = acc;
-        }
-    }
-    __syncthreads();
+// ------------------------------------------------------------------ G4 small fronts
+// One group of G threads per front (a warp for nf <= 32, several fronts per CTA; the whole CTA
+// above); the whole front lives in shared memory.  Fuses: extend-add of the children's update
+// blocks (G6), right-looking LDL' of the ns pivot columns with the reference's sign-based dynamic
+// regularisation (QDLDL semantics: if D[k]*sign < eps then D[k] = delta*sign), the inversion of the
+// diagonal blocks of L11 and the write-back of the L panel and of this front's update block.
+// Every entry sees the same floating-point operations in the same order as in the column-serial
+// schedule (per-entry order noted at each step), so the factor does not depend on G.
+// a warp group waits on its own named barrier (1 + its index in the CTA): __syncwarp() would bring
+// WARPSYNC.COLLECTIVE landing pads into the pivot loop
+template <int G>
+__device__ __forceinline__ void group_sync() {
+    if constexpr (G == 32) asm volatile("bar.sync %0, 32;" :: "r"(1 + (int)(threadIdx.x >> 5)) : "memory");
+    else __syncthreads();
 }
 
-// ------------------------------------------------------------------ G4 small fronts
-// One CTA per front; the whole front lives in shared memory.  Fuses: extend-add of the children's
-// update blocks (G6), right-looking LDL' of the ns pivot columns with the reference's sign-based
-// dynamic regularisation (QDLDL semantics: if D[k]*sign < eps then D[k] = delta*sign), and the
-// write-back of the L panel and of this front's update block.
-template <int THREADS>
-__global__ void __launch_bounds__(THREADS)
-k_factor_small(DevSym S, const int32_t* __restrict__ batch, double* __restrict__ Lst,
+template <int G, int FPC>
+__global__ void __launch_bounds__(G * FPC)
+k_factor_small(DevSym S, const int32_t* __restrict__ batch, int cnt, int fstride, double* __restrict__ Lst,
                double* __restrict__ Ust, double* __restrict__ D, double* __restrict__ Dinv,
                RegParams rp, unsigned int* __restrict__ nreg) {
-    extern __shared__ double F[];
-    const int s = batch[blockIdx.x];
+    static_assert(FPC == 1 || (G == 32 && FPC <= 15), "several fronts per CTA only with one warp per front");
+    extern __shared__ double smem_small[];
+    const int slot = blockIdx.x * FPC + (int)threadIdx.x / G;
+    if (slot >= cnt) return;                            // a whole group (FPC > 1: a whole warp)
+    double* F = smem_small + (size_t)((int)threadIdx.x / G) * fstride;
+    const int s = batch[slot];
     const int f = S.sn_first[s];
     const int ns = S.sn_first[s + 1] - f;
     const int nr = (int)(S.rows_ptr[s + 1] - S.rows_ptr[s]);
     const int nf = ns + nr;
-    const int tid = threadIdx.x;
+    const int tid = (int)threadIdx.x % G, lane = tid & 31, wid = tid >> 5;
+    constexpr int NW = G / 32;
     double* Lp = Lst + S.panel_off[s];
     // 1. panel -> first ns columns (identical layout), zero the trailing block
-    for (int i = tid; i < nf * ns; i += THREADS) F[i] = Lp[i];
-    for (int i = nf * ns + tid; i < nf * nf; i += THREADS) F[i] = 0.0;
-    __syncthreads();
-    // 2. extend-add, destination-owner form: warp w owns front columns d = w, w+NW, ...; the
-    // sources of a column are ordered by child => deterministic sums, no barrier per child
+    for (int i = tid; i < nf * ns; i += G) F[i] = Lp[i];
+    for (int i = nf * ns + tid; i < nf * nf; i += G) F[i] = 0.0;
+    group_sync<G>();
+    // 2. extend-add from the per-front child list, one child after the other with all threads: a child
+    // adds the lower triangle of its update block through rel (injective, so no two threads meet), and
+    // every entry is summed start + c1 + c2 ... in child_list order, the order of the destination-owner maps
     {
-        const int lane_ = tid & 31, wid_ = tid >> 5;
-        const int32_t* cp = S.asm_colptr + S.front_ptr[s];
-        const int64_t base = S.asm_base[s];
-        for (int d = wid_; d < nf; d += THREADS / 32) {
-            double* dst = F + d * nf;
-            for (int e = cp[d]; e < cp[d + 1]; ++e) {
-                const int q = S.asm_src[base + e];
-                const int c = S.asm_child[base + e];
-                const int64_t rp0 = S.rows_ptr[c];
-                const int nrc = (int)(S.rows_ptr[c + 1] - rp0);
-                const int j = (int)(q - rp0);
-                const int32_t* relc = S.rel + rp0;
-                const double* src = Ust + S.upd_off[c] + (int64_t)j * nrc;
-                for (int i = j + lane_; i < nrc; i += 32) dst[relc[i]] += src[i];
+        const int q0 = S.child_ptr[s], nch = S.child_ptr[s + 1] - q0;
+        Symbolic::KidEntry nxt{};
+        if (nch > 0) nxt = S.kids[q0];
+        for (int q = 0; q < nch; ++q) {
+            const Symbolic::KidEntry kd = nxt;
+            if (q + 1 < nch) nxt = S.kids[q0 + q + 1];
+            const int m = kd.nrc;
+            const int32_t* relc = S.rel + kd.roff;
+            const double* U = Ust + kd.uoff;
+            // thread tid takes entries tid, tid + G, ... of the lower triangle, column by column: column j
+            // holds rows j..m-1, so stepping past its end continues at row j+1 of column j+1
+            int i = tid, j = 0;
+            while (j < m && i >= m) { i -= m - j - 1; ++j; }
+            while (j < m) {
+                F[relc[i] + relc[j] * nf] += U[i + (int64_t)j * m];
+                i += G;
+                while (j < m && i >= m) { i -= m - j - 1; ++j; }
             }
+            group_sync<G>();
         }
-        __syncthreads();
     }
-    // 3. right-looking LDL' on the pivot columns
-    const int lane = tid & 31, wid = tid >> 5;
-    constexpr int NW = THREADS / 32;
-    for (int k = 0; k < ns; ++k) {
-        double d = F[k + k * nf];
-        const double sg = (double)S.dsign[f + k];
-        bool reg = false;
-        if (rp.enable && d * sg < rp.eps) { d = rp.delta * sg; reg = true; }
-        const double dinv = 1.0 / d;
-        const double* ck = F + k * nf;
-        for (int j = k + 1 + wid; j < nf; j += NW) {
-            const double wj = ck[j] * dinv;
-            double* cj = F + j * nf;
-            for (int i = j + lane; i < nf; i += 32) cj[i] -= ck[i] * wj;
-        }
-        __syncthreads();
-        for (int i = k + 1 + tid; i < nf; i += THREADS) F[i + k * nf] *= dinv;
-        if (tid == 0) {
-            F[k + k * nf] = d; D[f + k] = d; Dinv[f + k] = dinv;
-            if (reg) note_reg(rp, nreg, f + k);
-        }
-        __syncthreads();
-    }
-    // 3b. replace the diagonal blocks of L11 by their inverses (see invert_unit_lower_block)
+    // 3. right-looking LDL' on the pivot columns, one barrier per pivot: step k applies pivot k to the
+    // columns right of it (entry (i,j) -= F_ik * (F_jk * dinv_k), ascending k) and scales column k-1,
+    // which step k no longer reads
     {
-        double* buf = F + nf * nf;
-        for (int kb = 0; kb < ns; kb += SB) {
-            const int sb = min(SB, ns - kb);
-            if (sb > 1) invert_unit_lower_block(F + kb + kb * nf, nf, sb, buf, tid, THREADS);
+        double dp = 0.0, dinvp = 0.0;
+        bool regp = false;
+        for (int k = 0; k <= ns; ++k) {
+            if (k > 0) {
+                const int c = k - 1;
+                for (int i = k + tid; i < nf; i += G) F[i + c * nf] *= dinvp;
+                if (tid == 0) {
+                    F[c + c * nf] = dp; D[f + c] = dp; Dinv[f + c] = dinvp;
+                    if (regp) note_reg(rp, nreg, f + c);
+                }
+            }
+            if (k == ns) break;
+            double d = F[k + k * nf];
+            const double sg = (double)S.dsign[f + k];
+            bool reg = false;
+            if (rp.enable && d * sg < rp.eps) { d = rp.delta * sg; reg = true; }
+            const double dinv = 1.0 / d;
+            const double* ck = F + k * nf;
+            for (int j = k + 1 + wid; j < nf; j += NW) {
+                const double wj = ck[j] * dinv;
+                double* cj = F + j * nf;
+                for (int i = j + lane; i < nf; i += 32) cj[i] -= ck[i] * wj;
+            }
+            dp = d; dinvp = dinv; regp = reg;
+            group_sync<G>();
+        }
+        group_sync<G>();
+    }
+    // 3b. replace the diagonal blocks of L11 by their inverses in place (X = T^-1 for the solves' block
+    // GEMVs, see "inverted diagonal blocks" above).  T_ij is parked at the unused mirror position (j, i) and X_ij starts at
+    // -T_ij; step k subtracts T_ik X_kj from every X_ij with j < k < i, so each entry is
+    // -T_ij - sum_{k=j+1}^{i-1} T_ik X_kj accumulated in ascending k, with all threads on each step.
+    for (int kb = 0; kb < ns; kb += SB) {
+        const int sb = min(SB, ns - kb);
+        if (sb < 2) continue;
+        double* T = F + kb + kb * nf;
+        for (int e = tid; e < sb * sb; e += G) {
+            const int i = e % sb, j = e / sb;
+            if (i > j) { const double t = T[i + j * nf]; T[j + i * nf] = t; T[i + j * nf] = -t; }
+        }
+        group_sync<G>();
+        for (int k = 1; k < sb - 1; ++k) {
+            const int mi = sb - 1 - k;                  // rows k+1 .. sb-1
+            for (int e = tid; e < k * mi; e += G) {
+                const int i = k + 1 + e % mi, j = e / mi;
+                T[i + j * nf] -= T[k + i * nf] * T[k + j * nf];
+            }
+            group_sync<G>();
         }
     }
-    // 4. write back
-    for (int i = tid; i < nf * ns; i += THREADS) Lp[i] = F[i];
+    // 4. write back (the upper triangle of L11 is zero in the panel storage; the mirrors are dropped)
+    for (int e = tid; e < nf * ns; e += G) {
+        const int i = e % nf, j = e / nf;
+        Lp[e] = i < j ? 0.0 : F[e];
+    }
     if (nr > 0) {
         double* Us = Ust + S.upd_off[s];
         for (int j = wid; j < nr; j += NW) {

@@ -498,6 +498,11 @@ void symbolic_analyze(int64_t N64, const int64_t* colptr, const int64_t* rowval,
                 }
             }
         }
+        S.kids.resize(S.child_list.size());
+        for (size_t q = 0; q < S.child_list.size(); ++q) {
+            const int32_t c = S.child_list[q];
+            S.kids[q] = {S.upd_off[c], S.rows_ptr[c], S.nr(c), 0};
+        }
     }
     // scatter map of the original K entries into the panels
     S.a_map.resize(nnzK);

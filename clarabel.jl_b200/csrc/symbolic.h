@@ -75,6 +75,13 @@ struct Symbolic {
     std::vector<int32_t> asm_colptr;// [front_ptr.back()]
     std::vector<int32_t> asm_src;   // [rows_total minus roots]
     std::vector<int32_t> asm_child; // same length
+    // Per-front child lists of the shared-memory front kernel (k_factor_small): kids[child_ptr[s] + q]
+    // describes child child_list[child_ptr[s] + q] (its update block at Ust + uoff, nrc x nrc, and its
+    // rel at rel + roff).  rel is ascending, so a child adds the lower triangle of its update block to
+    // the rows and columns rel[] of the front; adding the children one after the other in this order
+    // sums every destination in the order of the destination-owner maps above.
+    struct KidEntry { int64_t uoff, roff; int32_t nrc, pad; };
+    std::vector<KidEntry> kids;     // [child_list.size()]
     std::vector<int32_t> sn_level;  // [nsuper]
     int32_t nlevels = 0;
     std::vector<int32_t> level_ptr; // [nlevels+1]

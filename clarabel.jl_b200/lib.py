@@ -194,6 +194,30 @@ class Symbolic:
         out["children"] = ch
         return out
 
+    def kid_lists(self):
+        """Per-front child lists of the shared-memory front kernel (cb200_symbolic_get selector 13):
+        [len(child_list), 3] of (update-block offset, rel offset, nr), row q for child_list[q]."""
+        L = lib()
+        cp = np.empty(self.stats["nsuper"] + 1, dtype=np.int64)
+        check(L.cb200_symbolic_get(self._h, 10, _p(cp), len(cp)), "cb200_symbolic_get")
+        out = np.empty(3 * int(cp[-1]), dtype=np.int64)
+        check(L.cb200_symbolic_get(self._h, 13, _p(out), len(out)), "cb200_symbolic_get")
+        return out.reshape(-1, 3)
+
+    def asm_maps(self):
+        """The destination-owner assembly maps (symbolic.h; selectors 14-18): front_ptr, asm_base,
+        asm_colptr, asm_src, asm_child"""
+        L = lib(); n = self.stats["nsuper"] + 1
+        out = {}
+        for sel, nm in ((14, "front_ptr"), (15, "asm_base")):
+            out[nm] = np.empty(n, dtype=np.int64)
+            check(L.cb200_symbolic_get(self._h, sel, _p(out[nm]), n), "cb200_symbolic_get")
+        for sel, nm, ln in ((16, "asm_colptr", out["front_ptr"][-1]), (17, "asm_src", out["asm_base"][-1]),
+                            (18, "asm_child", out["asm_base"][-1])):
+            out[nm] = np.empty(int(ln), dtype=np.int64)
+            check(L.cb200_symbolic_get(self._h, sel, _p(out[nm]), len(out[nm])), "cb200_symbolic_get")
+        return out
+
     def partition(self, nranks):
         n = self.stats["nsuper"]
         owner = np.empty(n, dtype=np.int64); top = np.empty(n, dtype=np.int64)

@@ -67,7 +67,11 @@ int64_t cb200_symbolic_stat(const cb200_symbolic* s, int32_t what);
 double  cb200_symbolic_flops(const cb200_symbolic* s);
 /* which: 0 perm[N], 1 sn_first[nsuper+1], 2 rows_ptr[nsuper+1], 3 rows[rows_total],
  *        4 rel[rows_total], 5 sn_parent[nsuper], 6 panel_off[nsuper+1], 7 upd_off[nsuper+1],
- *        8 a_map[nnzK], 9 sn_level[nsuper], 10 child_ptr[nsuper+1], 11 child_list[nsuper-#roots]
+ *        8 a_map[nnzK], 9 sn_level[nsuper], 10 child_ptr[nsuper+1], 11 child_list[nsuper-#roots],
+ *        12 panel_ld[nsuper], 13 per-front child lists [3 * (nsuper-#roots)]: (update-block offset,
+ *        rel offset, nr) of child_list[q] at 3q (symbolic.h, kids), the destination-owner assembly maps
+ *        14 front_ptr[nsuper+1], 15 asm_base[nsuper+1], 16 asm_colptr[front_ptr[nsuper]],
+ *        17 asm_src[asm_base[nsuper]], 18 asm_child[asm_base[nsuper]]
  * All arrays are returned widened to int64 into caller storage of the stated length. */
 int32_t cb200_symbolic_get(const cb200_symbolic* s, int32_t which, int64_t* out, int64_t len);
 /* Per-tile source lists of the large-front extend-add (symbolic.h, build_tile_lists) for the batch
